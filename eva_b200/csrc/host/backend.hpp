@@ -128,7 +128,8 @@ public:
     if (batch < 1 || batch > 65535 || replica < 0 || replica > 65535) throw std::invalid_argument("batch / replica out of range");
     const std::uint64_t key = planKey(batch, replica);
     auto h = std::static_pointer_cast<PlanHolder>(program.attachment(key));
-    if (!h || h->termCount != program.termCount() || h->opt.hoistModUp != options.hoistModUp || h->opt.approxHoist != options.approxHoist || h->opt.rotationChunk != options.rotationChunk) {   // stale plan: rebuilt
+    if (!h || h->termCount != program.termCount() || h->opt.hoistModUp != options.hoistModUp || h->opt.approxHoist != options.approxHoist || h->opt.rotationChunk != options.rotationChunk ||
+        h->opt.arenaLimit != options.arenaLimit) {   // stale plan: rebuilt
       h = std::make_shared<PlanHolder>();
       h->keepAlive = s_;
       ExecOptions o = options;

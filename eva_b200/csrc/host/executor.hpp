@@ -11,6 +11,7 @@
 // stream dependencies are events, and the whole replay can be captured into a
 // CUDA graph so that one execute() costs a single graph launch.
 #pragma once
+#include "arena_packer.hpp"
 #include "ckks_client.hpp"
 #include "ir.hpp"
 #include "logging.hpp"
@@ -100,6 +101,8 @@ struct ExecOptions {
   bool dedupTerms = true;      // identical ciphertext terms (same op, same attributes, same operands) are evaluated once and
                                // aliased: the compiled wide DAG of tests/large_programs.py style repeats each of its 127
                                // distinct rotations 64 times.  Same bits; still counted as executed IR terms.
+  std::size_t arenaLimit = 0;  // bytes a plan's arena may take (0: the free device memory at plan time).  A plan whose one-offset-per-
+                               // value layout exceeds it reuses the storage of dead values (arena_packer.hpp); over it even then: error
 };
 
 // scoped evab_set_batch: ops issued by this thread act on `batch` instances
@@ -133,8 +136,16 @@ public:
     long elided = 0;
     for (auto &t : order_) if ((t->op == Op::RotateLeftConst || t->op == Op::RotateRightConst) && vals_[t->index].fused) elided++;
     m["elided_rotations"] = elided;
+    m["arena_bytes"] = (long)arenaBytes(); m["arena_bytes_unpacked"] = (long)unpackedBytes_; m["packed"] = packed_ ? 1 : 0;
+    m["reuse_waits"] = reuseWaits_;
+    long constWords = 0;   // plaintexts of plan-time constants, resident for the plan's lifetime
+    if (opt_.cacheConstants)
+      for (auto &g : groups_) if (!g.dynamic) constWords += (long)g.members.size() * (g.ell + (g.withP ? 1 : 0)) * (long)N_;
+    m["constant_bytes"] = constWords * 8 * opt_.batch;
     return m;
   }
+  // false when the plan's arena is packed and the value's storage may have been reused by a later value of the run
+  bool intact(std::uint64_t index) const { return !packed_ || keptAfterRun_.at(index); }
   // private stream used by B200Public::execute for H2D -> run -> D2H of this plan,
   // so that execute() calls on different programs overlap on the GPU
   std::size_t arenaBytes() const { return (stride_ * (std::size_t)opt_.batch + 8 + rawStride_ * (std::size_t)opt_.batch + 8) * 8; }
@@ -640,6 +651,16 @@ private:
     for (int s = 0; s < usedStreams_; s++) { workOff_[s] = arenaWords; arenaWords += workWords[s]; }
     stride_ = (arenaWords + 63) & ~std::size_t(63);
     rawStride_ = (rawWords_ + 7) & ~std::size_t(7);
+    // ---- arena layout: one offset per value (above) when it fits the limit, else the storage of dead values is reused
+    unpackedBytes_ = arenaBytes();
+    std::size_t limit = opt_.arenaLimit;
+    if (!limit) { std::size_t freeB = 0, totalB = 0; check(evab_mem_info(dev_->ctx(), &freeB, &totalB)); limit = freeB; }
+    if (unpackedBytes_ > limit) {
+      packLayout(hoistSrc, workWords, stepOperands);
+      if (arenaBytes() > limit)
+        throw std::runtime_error("plan arena needs " + std::to_string(arenaBytes()) + " bytes packed (" + std::to_string(unpackedBytes_) +
+                                 " bytes unpacked), more than the limit of " + std::to_string(limit) + " bytes");
+    }
     arena_ = DBuf(dev_, stride_ * opt_.batch + 8);
     rawArena_ = DBuf(dev_, rawStride_ * opt_.batch + 8);
     dev_->sync();  // stream-ordered allocation made on the null stream: publish it to the plan's streams
@@ -696,6 +717,122 @@ private:
         }
       }
     if (numFlags_) check(evab_host_alloc(8 * numFlags_ * 8 * (std::size_t)opt_.batch, (void **)&hostFlags_));
+  }
+  // Packed arena: describes every region of the plan to packArena (one buffer per materialised value; one per rotation chunk,
+  // lazy rotation sum, encode group and hoist group covering all their members), then moves every offset to the packed
+  // layout and adds the write-after-read waits it asks for.  Steps, launches and their operands' values are unchanged.
+  template <class StepOperands>
+  void packLayout(const std::vector<const Term *> &hoistSrc, const std::vector<std::size_t> &workWords, StepOperands stepOperands) {
+    const std::uint64_t TC = prog_.termCount();
+    const std::size_t H = hoistSrc.size(), L = lazy_.size();
+    const int nSteps = (int)steps_.size();
+    std::unordered_map<std::uint64_t, int> stepOf;   // producer -> step
+    std::vector<int> stepOfEvent(numEvents_, -1);
+    for (int i = 0; i < nSteps; i++) {
+      stepOf[steps_[i].producer] = i;
+      if (steps_[i].record >= 0) stepOfEvent[steps_[i].record] = i;
+    }
+    std::vector<PackStep> ps(nSteps);
+    for (int i = 0; i < nSteps; i++) {
+      ps[i].stream = steps_[i].stream;
+      for (int e : steps_[i].waits) if (stepOfEvent[e] >= 0) ps[i].waits.push_back(stepOfEvent[e]);
+    }
+    std::vector<PackBuffer> pb;
+    auto newBuf = [&](std::size_t words, int writer, bool pinned) {
+      pb.push_back(PackBuffer{(words + 63) & ~std::size_t(63), writer, {}, pinned});   // 512-byte aligned, like the unpacked stride
+      return (int)pb.size() - 1;
+    };
+    auto writerOf = [&](std::uint64_t producer) { auto f = stepOf.find(producer); return f == stepOf.end() ? -1 : f->second; };
+    std::vector<int> bufOfVal(TC, -1), hoistBuf(H, -1), lazyBuf(L, -1), chunkBuf(chunks_.size(), -1), groupBuf(groups_.size(), -1);
+    for (auto &t : order_) {
+      const ValueInfo &v = vals_[t->index];
+      if ((v.kind != Kind::Cipher && v.kind != Kind::Plain) || v.alias || v.fused || t->op == Op::Encode || chunkOf_.count(t->index)) continue;
+      const std::size_t words = (std::size_t)(v.kind == Kind::Cipher ? v.size : 1) * v.ell * N_;
+      bufOfVal[t->index] = t->op == Op::Input ? newBuf(words, 0, true) : newBuf(words, stepOf.at(t->index), false);
+    }
+    auto extWords = [&](int ell) { return opt_.hoistModUp ? evab_rotate_modup_ext_bytes(dev_->ctx(), ell) / 8 : 0; };
+    for (std::size_t g = 0; g < H; g++) {
+      const int ell = vals_[hoistSrc[g]->index].ell;
+      if (int w = writerOf(TC + g); w >= 0) hoistBuf[g] = newBuf((std::size_t)ell * N_ + extWords(ell), w, false);
+    }
+    for (std::size_t l = 0; l < L; l++) lazyBuf[l] = newBuf(lazy_[l].roots.size() * 2 * (std::size_t)lazy_[l].ell * N_, stepOf.at(TC + H + l), false);
+    for (std::size_t c = 0; c < chunks_.size(); c++) chunkBuf[c] = newBuf(chunks_[c].rots.size() * 2 * (std::size_t)chunks_[c].ell * N_, stepOf.at(TC + H + L + c), false);
+    auto groupPlainWords = [&](const EncodeGroup &g) { return (std::size_t)(g.ell + (g.withP ? 1 : 0)) * N_; };
+    for (std::size_t g = 0; g < groups_.size(); g++) {
+      const EncodeGroup &G = groups_[g];
+      const std::size_t words = G.members.size() * groupPlainWords(G) + evab_encode_work_bytes(dev_->ctx(), (int)G.members.size() - G.nUniform) / 8;
+      groupBuf[g] = newBuf(words, stepOf.at(G.first->index), !G.dynamic && opt_.cacheConstants);   // cached constants: encoded at plan time
+    }
+    const int flagsBuf = numFlags_ ? newBuf(8 * numFlags_, 0, true) : -1;
+    std::vector<int> workBuf(usedStreams_);
+    for (int s = 0; s < usedStreams_; s++) workBuf[s] = newBuf(workWords[s], 0, true);
+    // storage of a term: aliases (Output, duplicate terms) resolve to their source; chunk members and encode members to their composite
+    auto bufOfTerm = [&](std::uint64_t x) -> int {
+      while (vals_[x].alias) x = aliasSource(byIndex_[x]);
+      if (vals_[x].kind != Kind::Cipher && vals_[x].kind != Kind::Plain) return -1;
+      if (auto c = chunkOf_.find(x); c != chunkOf_.end()) return chunkBuf[c->second];
+      if (byIndex_[x]->op == Op::Encode) return groupBuf[groupIndex_.at(x)];
+      return bufOfVal[x];
+    };
+    auto read = [&](int step, int b) { if (b >= 0) pb[b].readers.push_back(step); };
+    for (int i = 0; i < nSteps; i++) {
+      const Step &st = steps_[i];
+      const std::uint64_t src = st.term->index;
+      if (st.op == Op::Undef) {   // pseudo steps (hoist, rotation chunk, lazy rotation sums) read the group's source
+        read(i, bufOfTerm(src));
+        if (st.chunk >= 0) read(i, hoistBuf[chunks_[st.chunk].gid]);
+        if (st.lazy >= 0) {
+          read(i, hoistBuf[lazy_[st.lazy].gid]);
+          for (auto &ws : lazy_[st.lazy].wts) for (const Term *w : ws) if (w) read(i, bufOfTerm(w->index));
+        }
+        continue;
+      }
+      for (const Term *o : stepOperands(st.term)) read(i, bufOfTerm(o->index));   // a fused sum reads its leaves
+      if (auto lz = lazyOfRoot_.find(src); lz != lazyOfRoot_.end()) for (auto &lo : lz->second) read(i, lazyBuf[lo.first]);
+      if (st.hoist >= 0) read(i, hoistBuf[st.hoist]);
+    }
+    for (auto &o : prog_.getOutputs()) if (int b = bufOfTerm(o.second->index); b >= 0) pb[b].pinned = true;   // downloaded after the run
+
+    const PackResult pr = packArena(ps, pb);
+    auto at = [&](int b) { return pr.offsets.at(b); };
+    for (auto &t : order_) if (bufOfVal[t->index] >= 0) vals_[t->index].off = at(bufOfVal[t->index]);
+    for (std::size_t g = 0; g < H; g++)
+      if (hoistBuf[g] >= 0) {
+        hoistOff_[g] = at(hoistBuf[g]);
+        if (opt_.hoistModUp) hoistExtOff_[g] = hoistOff_[g] + (std::size_t)vals_[hoistSrc[g]->index].ell * N_;
+      }
+    for (std::size_t l = 0; l < L; l++) lazy_[l].tempOff = at(lazyBuf[l]);
+    for (std::size_t c = 0; c < chunks_.size(); c++) {
+      RotChunk &ch = chunks_[c];
+      ch.outOff = at(chunkBuf[c]);
+      for (std::size_t i = 0; i < ch.rots.size(); i++) vals_[ch.rots[i]->index].off = ch.outOff + i * 2 * (std::size_t)ch.ell * N_;
+    }
+    for (std::size_t g = 0; g < groups_.size(); g++) {
+      EncodeGroup &G = groups_[g];
+      G.outOff = at(groupBuf[g]);
+      for (std::size_t i = 0; i < G.members.size(); i++) vals_[G.members[i]->index].off = G.outOff + i * groupPlainWords(G);
+      G.workOff = G.outOff + G.members.size() * groupPlainWords(G);
+    }
+    for (auto &kv : encodeAlias_) vals_[kv.first].off = vals_[kv.second->index].off;
+    if (flagsBuf >= 0) flagsOff_ = at(flagsBuf);
+    for (int s = 0; s < usedStreams_; s++) workOff_[s] = at(workBuf[s]);
+    for (auto &t : order_) if (vals_[t->index].alias) vals_[t->index].off = vals_[aliasSource(t)].off;
+    for (auto &st : steps_) {
+      if (st.lazyTemps.empty()) continue;
+      st.lazyTemps.clear();
+      for (auto &lo : lazyOfRoot_.at(st.term->index)) st.lazyTemps.push_back(lazy_[lo.first].tempOff + (std::size_t)lo.second * 2 * lazy_[lo.first].ell * N_);
+    }
+    for (auto &w : pr.waits) {   // write-after-read edges: the reusing step waits on the event of the last reader
+      Step &last = steps_[w.second];
+      if (last.record < 0) last.record = numEvents_++;
+      std::vector<int> &waits = steps_[w.first].waits;
+      if (std::find(waits.begin(), waits.end(), last.record) == waits.end()) waits.push_back(last.record);
+    }
+    reuseWaits_ = (long)pr.waits.size();
+    keptAfterRun_.assign(TC, 0);
+    for (auto &t : order_) if (int b = bufOfTerm(t->index); b >= 0) keptAfterRun_[t->index] = pb[b].pinned;
+    stride_ = (pr.peak + 63) & ~std::size_t(63);
+    packed_ = true;
   }
   // canonical (first) occurrence of a term that repeats an earlier one (dedupTerms)
   const Term *C(const Term *t) const { return byIndex_[canon_[t->index]]; }
@@ -981,6 +1118,10 @@ private:
   bool graphValid_ = false, rawDirty_ = false, rawInputs_ = false, hasDynamicEncodes_ = false;
   int numEvents_ = 0, usedStreams_ = 0;
   std::size_t cipherOps_ = 0;
+  bool packed_ = false;                  // arena laid out by packArena (storage of dead values reused)
+  std::size_t unpackedBytes_ = 0;        // arenaBytes() of the one-offset-per-value layout
+  long reuseWaits_ = 0;                  // event waits packArena added
+  std::vector<char> keptAfterRun_;       // packed plan: term index -> its storage is pinned (inputs, outputs, cached constants)
   DBuf arena_;
 };
 

@@ -91,6 +91,17 @@ PYBIND11_MODULE(_eva_b200, m) {
       .def("_make_output", &Program::makeOutput, py::keep_alive<0, 1>());
 
   m.def("evaluate", &evaluate, py::arg("program"), py::arg("inputs"), "Evaluate the program without homomorphic encryption");
+  // test hook: the arena packer alone (host/arena_packer.hpp).  steps: [(stream, [earlier steps waited on])];
+  // buffers: [(words, writer step, [reader steps], pinned)] -> (offsets, added waits [(step, earlier step)], peak words)
+  m.def("_pack_arena", [](const std::vector<std::tuple<int, std::vector<int>>> &steps,
+                          const std::vector<std::tuple<std::size_t, int, std::vector<int>, bool>> &buffers) {
+    std::vector<PackStep> ps;
+    for (auto &s : steps) ps.push_back(PackStep{std::get<0>(s), std::get<1>(s)});
+    std::vector<PackBuffer> pb;
+    for (auto &b : buffers) pb.push_back(PackBuffer{std::get<0>(b), std::get<1>(b), std::get<2>(b), std::get<3>(b)});
+    PackResult r = packArena(ps, pb);
+    return py::make_tuple(r.offsets, r.waits, r.peak);
+  }, py::arg("steps"), py::arg("buffers"));
   m.def("set_num_threads", [](int) {}, py::arg("num_threads"),
         "Kept for API compatibility: the DAG is scheduled on CUDA streams, not CPU threads.");
   py::class_<int>(m, "_GaloisGuard").def(py::init());
@@ -172,13 +183,17 @@ PYBIND11_MODULE(_eva_b200, m) {
              { py::gil_scoped_release rel; outs = p.collect(*h->batch); }
              return outs;
            }, py::arg("handle"))
-      .def("set_options", [](B200Public &p, int streams, bool graph, bool cache, bool dedup, int fuse, bool fuseSums, bool hoist, bool uniformEncode, bool dedupTerms, bool hoistModUp, bool approxHoist, int rotationChunk) {
+      .def("set_options", [](B200Public &p, int streams, bool graph, bool cache, bool dedup, int fuse, bool fuseSums, bool hoist, bool uniformEncode, bool dedupTerms, bool hoistModUp, bool approxHoist, int rotationChunk, std::size_t arenaLimit) {
              p.options.numStreams = streams; p.options.useGraph = graph; p.options.cacheConstants = cache; p.options.dedupConstants = dedup;
              p.options.fuse = fuse; p.options.fuseSums = fuseSums; p.options.hoistRotations = hoist; p.options.uniformEncode = uniformEncode;
              p.options.dedupTerms = dedupTerms; p.options.hoistModUp = hoistModUp; p.options.approxHoist = approxHoist; p.options.rotationChunk = rotationChunk;
+             p.options.arenaLimit = arenaLimit;
            },
            py::arg("num_streams") = 8, py::arg("use_graph") = true, py::arg("cache_constants") = true, py::arg("dedup_constants") = true,
-           py::arg("fuse") = 1, py::arg("fuse_sums") = true, py::arg("hoist_rotations") = true, py::arg("uniform_encode") = true, py::arg("dedup_terms") = true, py::arg("hoist_mod_up") = true, py::arg("approx_hoist") = false, py::arg("rotation_chunk") = 16)
+           py::arg("fuse") = 1, py::arg("fuse_sums") = true, py::arg("hoist_rotations") = true, py::arg("uniform_encode") = true, py::arg("dedup_terms") = true, py::arg("hoist_mod_up") = true, py::arg("approx_hoist") = false, py::arg("rotation_chunk") = 16,
+           py::arg("arena_limit") = 0,
+           "arena_limit: bytes one plan's arena may take (0: the free device memory when the plan is built).  A plan whose one-offset-per-value "
+           "layout does not fit reuses the storage of dead values; if even that exceeds the limit, building the plan raises RuntimeError")
       .def("set_input_sizes", [](B200Public &p, const std::map<std::string, int> &sizes) { p.options.inputSizes = sizes; },
            "ciphertext inputs that are not size 2 (name -> polynomials); applies to plans built afterwards")
       .def("drop_plan", &B200Public::dropExecutor, py::arg("program"), py::arg("batch") = 1, py::arg("replica") = 0)
@@ -267,6 +282,9 @@ PYBIND11_MODULE(_eva_b200, m) {
         auto dev = p.shared()->dev;
         if (vi.kind == Kind::Raw) return py::cast(ex.rawValue(index, b));
         if (vi.kind == Kind::None || vi.fused) return py::none();   // fused away: never materialised
+        if (!ex.intact(index))
+          throw std::runtime_error("term " + std::to_string(index) + " is not kept by this plan's packed arena (its storage is reused after its last "
+                                   "use); only inputs, outputs and cached constants can be read back");
         const std::size_t polys = vi.kind == Kind::Cipher ? vi.size : 1;
         u64arr a({polys, (std::size_t)vi.ell, (std::size_t)dev->N()});
         dev->sync();
