@@ -49,6 +49,8 @@ _SIGS = {
     "evab_rotate_modup_scale_c0": (ci, [vp, ci, vp, vp, vp]),
     "evab_rotate_modup_many_work_bytes": (szt, [vp, ci, ci]),
     "evab_rotate_modup_many": (ci, [vp, ci, ci, vp, vp, vp, vp, vp, vp, vp, vp]),
+    "evab_rotate_wsum_work_bytes": (szt, [vp, ci, ci, ci]),
+    "evab_rotate_wsum": (ci, [vp, ci, ci, vp, vp, vp, ci, vp, vp, vp, vp, ci, vp, vp, vp, vp]),
     "evab_lazy_rotsum_work_bytes": (szt, [vp, ci, ci]),
     "evab_lazy_rotsum": (ci, [vp, ci, ci, vp, vp, vp, ci, vp, vp, vp, vp, vp, vp]),
     "evab_encode_ext": (ci, [vp, ci, vp, vp, vp, ci, ci, vp, vp, vp]),

@@ -209,6 +209,12 @@ __global__ void __launch_bounds__(256, 4) k_rot_many(const RotManyArgs A, const 
   const int i = blockIdx.y / (A.ell + 1), mi = blockIdx.y % (A.ell + 1);
   for (int j = (blockIdx.x * blockDim.x + threadIdx.x) * 2; j < A.N; j += gridDim.x * blockDim.x * 2) rot_many_elem(A, i, mi, j, off);
 }
+// grid.y = (polynomial, residue) of the outputs
+__global__ void __launch_bounds__(256) k_rot_wsum(const WsumArgs A, const long long bstride) {
+  const long long off = (long long)blockIdx.z * bstride;
+  const int c = blockIdx.y / A.ell, r = blockIdx.y % A.ell;
+  for (int j = (blockIdx.x * blockDim.x + threadIdx.x) * 2; j < A.N; j += gridDim.x * blockDim.x * 2) rot_wsum_elem(A, c, r, j, off);
+}
 // block = 32 element pairs x n rotations (one warp per rotation); the parts meet in shared memory, one output sum at a time
 __global__ void __launch_bounds__(32 * LRS_MAX) k_lazy_rotsum(const LazyRotSumArgs A, const long long bstride) {
   __shared__ u64 sh[LRS_MAX][4][32];
@@ -322,6 +328,7 @@ template <int LOGN, int CL, int AR> static int launch_fwd_c(const NttLaunch &L, 
   if (L.pro == PRO_MODRED && L.epi == EPI_STORE) return launch_fwd_m<LOGN, PRO_MODRED, EPI_STORE, CL, AR>(L, jobs, st);
   if (L.pro == PRO_MODRED && L.epi == EPI_STORE_LAZY) return launch_fwd_m<LOGN, PRO_MODRED, EPI_STORE_LAZY, CL, AR>(L, jobs, st);
   if (L.pro == PRO_MODRED && L.epi == EPI_DIVROUND) return launch_fwd_m<LOGN, PRO_MODRED, EPI_DIVROUND, CL, AR>(L, jobs, st);
+  if (L.pro == PRO_PLAIN && L.epi == EPI_DIVROUND) return launch_fwd_m<LOGN, PRO_PLAIN, EPI_DIVROUND, CL, AR>(L, jobs, st);
   if (L.pro == PRO_MODRED_SG && L.epi == EPI_STORE_LAZY) return launch_fwd_m<LOGN, PRO_MODRED_SG, EPI_STORE_LAZY, CL, AR>(L, jobs, st);
   return fail("unsupported forward NTT prologue/epilogue combination");
 }
@@ -444,6 +451,12 @@ struct CudaBE {
   int rot_many(const RotManyArgs &A) {
     count();
     k_rot_many<<<grid(A.n * (A.ell + 1)), 256, 0, st>>>(A, g_batch.stride);
+    CUDA_OK(cudaGetLastError());
+    return 0;
+  }
+  int rot_wsum(const WsumArgs &A) {
+    count();
+    k_rot_wsum<<<grid(2 * A.ell), 256, 0, st>>>(A, g_batch.stride);
     CUDA_OK(cudaGetLastError());
     return 0;
   }
@@ -847,6 +860,19 @@ extern "C" int evab_lazy_rotsum(evab_ctx *c, int ell, int nout, uint64_t *o, con
     perms[i] = perm;
   }
   BE_BEGIN return lazy_rotsum_impl(be, c->v, ell, nout, o, a, ext, n, perms, keys, cadds, wts, (u64 *)work);
+}
+extern "C" size_t evab_rotate_wsum_work_bytes(const evab_ctx *c, int ell, int n, int nout) { return rotate_wsum_work_elems(c->v, ell, n, nout) * sizeof(u64); }
+extern "C" int evab_rotate_wsum(evab_ctx *c, int ell, int nout, uint64_t *o, const uint64_t *a, const uint64_t *ext, int n, const uint64_t *elts,
+                                const uint64_t *const *keys, const uint64_t *const *cadds, const uint64_t *const *wts, int ntap,
+                                const uint64_t *const *taps, const uint64_t *const *twts, void *work, void *stream) {
+  if (n < 1 || n > WS_MAX) return fail("evab_rotate_wsum: 1..16 rotations");
+  const u32 *perms[WS_MAX];
+  for (int i = 0; i < n; i++) {
+    u32 *perm = nullptr, *ctab = nullptr;
+    if (galois_tables(c, elts[i], &perm, &ctab, "evab_rotate_wsum")) return 1;
+    perms[i] = perm;
+  }
+  BE_BEGIN return rotate_wsum_impl(be, c->v, ell, nout, o, a, ext, n, perms, keys, cadds, wts, ntap, taps, twts, (u64 *)work);
 }
 extern "C" int evab_memset_zero(evab_ctx *c, void *d, size_t bytes, void *stream) {
   CUDA_OK(cudaSetDevice(c->device));

@@ -129,6 +129,7 @@ public:
     const std::uint64_t key = planKey(batch, replica);
     auto h = std::static_pointer_cast<PlanHolder>(program.attachment(key));
     if (!h || h->termCount != program.termCount() || h->opt.hoistModUp != options.hoistModUp || h->opt.approxHoist != options.approxHoist || h->opt.rotationChunk != options.rotationChunk ||
+        h->opt.rotationSums != options.rotationSums ||
         h->opt.arenaLimit != options.arenaLimit) {   // stale plan: rebuilt
       h = std::make_shared<PlanHolder>();
       h->keepAlive = s_;

@@ -52,7 +52,7 @@ struct Step {
   std::vector<int> sumKind;    // per leaf: 0 ciphertext, 1 ciphertext * plaintext, 2 ciphertext (x) ciphertext
   int hoist = -1;              // rotation group sharing one inverse NTT (op == Undef: the step computing it)
   std::uint64_t producer = 0;  // term index, or termCount + group for a hoist step
-  int lazy = -1;               // approxHoist: index of the lazy rotation sums this pseudo step computes (op == Undef)
+  int lazy = -1;               // approxHoist / rotationSums: index of the rotation sums this pseudo step computes (op == Undef)
   int chunk = -1;              // rotationChunk: index of the rotation chunk this pseudo step computes (op == Undef)
   std::vector<std::size_t> lazyTemps;  // fused sum: arena offsets of the lazy rotation sums added to the other leaves
 };
@@ -72,12 +72,15 @@ struct RotChunk {
   std::size_t outOff = 0;                           // their results, contiguous: [n][2][ell][N]
   bool emitted = false;
 };
-// approxHoist: out_o = sum_i wts[o][i] (.) rots[i] over rotations of one hoist group, each sum rounded down by P once (evab_lazy_rotsum)
+// approxHoist: out_o = sum_i wts[o][i] (.) rots[i] over rotations of one hoist group, each sum rounded down by P once (evab_lazy_rotsum);
+// rotationSums: the same sums with scalar-constant weights and every rotation rounded on its own, + sum_t twts[o][t] (.) taps[t] (evab_rotate_wsum)
 struct LazySum {
   int gid = 0, ell = 0;
   std::vector<const Term *> rots;                   // union of the rotations (never materialised when all their uses are lazy)
   std::vector<const Term *> roots;                  // the fused sum every output feeds
   std::vector<std::vector<const Term *>> wts;       // [output][rotation]: plaintext weight, null when the rotation is not in that sum
+  std::vector<const Term *> taps;                   // rotationSums: size-2 ciphertexts of the sums' other scalar-weighted leaves
+  std::vector<std::vector<const Term *>> twts;      // [output][tap]: their weights, null when the tap is not in that sum
   std::size_t tempOff = 0;                          // arena offset of the outputs [nout][2][ell][N]
   bool emitted = false, allStatic = true;
 };
@@ -97,6 +100,8 @@ struct ExecOptions {
   int rotationChunk = 16;      // with hoistModUp: rotations of one ciphertext computed per evab_rotate_modup_many call (same bits); < 2: one call each
   bool approxHoist = false;    // OPT-IN, NOT bit-exact (SURVEY 8f-4): sums of plaintext-weighted rotations of one ciphertext are rounded down by P
                                // once per sum instead of once per rotation (evab_lazy_rotsum); graded by the MSE criterion only
+  bool rotationSums = true;    // with hoistModUp and fuseSums: leaves "rotation of a hoist group (x) scalar constant" of fused sums are summed by
+                               // evab_rotate_wsum (same bits, 2 n + 2 nout ell transforms instead of n (2 + 2 ell)); approxHoist takes precedence
   bool dedupConstants = true;  // Encode terms of identical constants at the same (level, scale) share one plaintext
   bool dedupTerms = true;      // identical ciphertext terms (same op, same attributes, same operands) are evaluated once and
                                // aliased: the compiled wide DAG of tests/large_programs.py style repeats each of its 127
@@ -130,8 +135,15 @@ public:
   std::map<std::string, long> planStats() const {
     std::map<std::string, long> m;
     m["steps"] = (long)steps_.size(); m["streams"] = usedStreams_; m["hoist_groups"] = (long)hoistOff_.size();
-    m["rotation_chunks"] = (long)chunks_.size(); m["lazy_sums"] = 0; m["lazy_calls"] = (long)lazy_.size(); m["lazy_rotations"] = 0; m["chunked_rotations"] = 0;
-    for (auto &L : lazy_) { m["lazy_sums"] += (long)L.roots.size(); m["lazy_rotations"] += (long)L.rots.size(); }
+    m["rotation_chunks"] = (long)chunks_.size(); m["chunked_rotations"] = 0;
+    const bool approx = opt_.approxHoist;   // lazy_ holds the approximate (lazy_*) or the exact (rotation_sum_*) calls
+    m["lazy_calls"] = approx ? (long)lazy_.size() : 0; m["rotation_sum_calls"] = approx ? 0 : (long)lazy_.size();
+    m["lazy_sums"] = m["lazy_rotations"] = m["rotation_sums"] = m["rotation_sum_rotations"] = m["rotation_sum_taps"] = 0;
+    for (auto &L : lazy_) {
+      m[approx ? "lazy_sums" : "rotation_sums"] += (long)L.roots.size();
+      m[approx ? "lazy_rotations" : "rotation_sum_rotations"] += (long)L.rots.size();
+      m["rotation_sum_taps"] += (long)L.taps.size();
+    }
     for (auto &c : chunks_) m["chunked_rotations"] += (long)c.rots.size();
     long elided = 0;
     for (auto &t : order_) if ((t->op == Op::RotateLeftConst || t->op == Op::RotateRightConst) && vals_[t->index].fused) elided++;
@@ -377,12 +389,34 @@ private:
         for (const Term *r : kv.second) hoistOf[r->index] = gid;
       }
     }
-    // ---- approxHoist (opt-in): leaves "rotation of a hoist group (x) constant plaintext" of a fused sum, two or more of the same
-    // group, become ONE lazy rotation sum whose temporary joins the remaining leaves; a rotation all of whose uses went that way is
-    // never materialised.  The plaintexts involved are encoded with an extra residue row mod P.
-    if (opt_.approxHoist && opt_.hoistModUp && opt_.fuseSums) {
-      std::vector<int> usesAll(prog_.termCount(), 0), lazyUses(prog_.termCount(), 0);
+    // ---- rotation sums.  approxHoist (opt-in): leaves "rotation of a hoist group (x) constant plaintext" of a fused sum, two or more
+    // of the same group, become ONE lazy rotation sum whose temporary joins the remaining leaves; a rotation all of whose uses went that
+    // way is never materialised.  The plaintexts involved are encoded with an extra residue row mod P.
+    // rotationSums (exact, evab_rotate_wsum): the same grouping, for rotations whose every use is such a leaf with a scalar constant
+    // weight.  A leaf of weight 0.0 is dropped (its product is the zero ciphertext), and the sum's other leaves "size-2 ciphertext
+    // (x) scalar constant" join the call as taps (a rotation by 0 through its operand).  A sum left with no other leaf is the call's
+    // output itself: it is never issued as a step of its own.
+    const bool exactSums = !opt_.approxHoist && opt_.rotationSums;
+    if ((opt_.approxHoist || exactSums) && opt_.hoistModUp && opt_.fuseSums) {
+      std::vector<int> usesAll(prog_.termCount(), 0), lazyUses(prog_.termCount(), 0), wsumLeaves(prog_.termCount(), 0), pos(prog_.termCount(), 0);
       for (auto &t : order_) if (canon_[t->index] == t->index) for (auto &o : t->getOperands()) usesAll[canon_[o->index]]++;
+      for (std::size_t i = 0; i < order_.size(); i++) pos[order_[i]->index] = (int)i;
+      // a replicated scalar constant (the uniform encoder's predicate) and its value
+      auto scalarWeight = [&](const Term *pt, double &v) {
+        if (pt->op != Op::Encode || pt->operandAt(0)->op != Op::Constant) return false;
+        const auto &x = rawsB_[0][pt->operandAt(0)->index];
+        if (x.empty() || !std::all_of(x.begin(), x.end(), [&](double y) { return std::memcmp(&y, &x[0], sizeof(double)) == 0; })) return false;
+        v = x[0];
+        return true;
+      };
+      auto rotLeaf = [&](const std::pair<const Term *, const Term *> &l) {
+        double v;
+        return hoistOf.count(l.first->index) && vals_[l.first->index].size == 2 && (exactSums ? scalarWeight(l.second, v) : l.second->op == Op::Encode);
+      };
+      if (exactSums)
+        for (auto &kv : sumOf)
+          for (std::size_t i = 0; i < kv.second.size(); i++)
+            if (sumKindOf.at(kv.first)[i] == 1 && rotLeaf(kv.second[i])) wsumLeaves[kv.second[i].first->index]++;
       std::map<int, int> openOf;   // hoist group -> the lazy sum that still takes outputs
       for (auto &t : order_) {
         auto f = sumOf.find(t->index);
@@ -391,18 +425,18 @@ private:
         auto &kinds = sumKindOf.at(t->index);
         std::map<int, std::vector<int>> byGroup;
         for (int i = 0; i < (int)leaves.size(); i++) {
-          if (kinds[i] != 1) continue;
-          auto h = hoistOf.find(leaves[i].first->index);
-          if (h == hoistOf.end() || leaves[i].second->op != Op::Encode || vals_[leaves[i].first->index].size != 2) continue;
-          byGroup[h->second].push_back(i);
+          if (kinds[i] != 1 || !rotLeaf(leaves[i])) continue;
+          if (exactSums && wsumLeaves[leaves[i].first->index] != usesAll[leaves[i].first->index]) continue;
+          byGroup[hoistOf.at(leaves[i].first->index)].push_back(i);
         }
+        auto isZero = [&](int i) { double v = 1.0; return exactSums && scalarWeight(leaves[i].second, v) && v == 0.0; };
         std::vector<char> drop(leaves.size(), 0);
         std::vector<std::pair<int, std::vector<int>>> slices;   // at most 16 rotations per call: longer sums are cut
         for (auto &kv : byGroup)
           for (std::size_t b = 0; b < kv.second.size(); b += 16)
             slices.emplace_back(kv.first, std::vector<int>(kv.second.begin() + b, kv.second.begin() + std::min(kv.second.size(), b + 16)));
         for (auto &kv : slices) {
-          if (kv.second.size() < 2) continue;
+          if (kv.second.size() < 2 || std::all_of(kv.second.begin(), kv.second.end(), isZero)) continue;
           // sums over rotations of the same ciphertext share one call (and the inner products of the rotations they have in
           // common), as long as the later sum's weights are available when the first one runs
           int li = -1;
@@ -412,7 +446,7 @@ private:
             std::size_t extra = 0;
             bool ready = L.roots.size() < 4 && L.allStatic;
             for (int i : kv.second) {
-              if (std::find(L.rots.begin(), L.rots.end(), leaves[i].first) == L.rots.end()) extra++;
+              if (!isZero(i) && std::find(L.rots.begin(), L.rots.end(), leaves[i].first) == L.rots.end()) extra++;
               if (leaves[i].second->operandAt(0)->op != Op::Constant) ready = false;
             }
             if (ready && L.rots.size() + extra <= 16) li = op->second;
@@ -427,24 +461,51 @@ private:
           L.roots.push_back(t);
           for (auto &w : L.wts) w.resize(L.rots.size(), nullptr);
           L.wts.emplace_back(L.rots.size(), nullptr);
+          L.twts.emplace_back(L.taps.size(), nullptr);
           for (int i : kv.second) {
+            if (isZero(i)) { drop[i] = 1; lazyUses[leaves[i].first->index]++; continue; }
             auto r = std::find(L.rots.begin(), L.rots.end(), leaves[i].first);
             if (r == L.rots.end()) { L.rots.push_back(leaves[i].first); for (auto &w : L.wts) w.push_back(nullptr); r = L.rots.end() - 1; }
             auto &slot = L.wts.back()[r - L.rots.begin()];
             if (slot) continue;   // the same rotation twice in one sum: the second one stays an ordinary leaf
             slot = leaves[i].second;
             if (slot->operandAt(0)->op != Op::Constant) L.allStatic = false;
-            drop[i] = 1; lazyUses[leaves[i].first->index]++; needP_.insert(leaves[i].second->index);
+            drop[i] = 1; lazyUses[leaves[i].first->index]++;
+            if (!exactSums) needP_.insert(leaves[i].second->index);
           }
           lazyOfRoot_[t->index].emplace_back(li, (int)L.roots.size() - 1);
         }
-        if (lazyOfRoot_.count(t->index)) {
-          std::vector<std::pair<const Term *, const Term *>> keep; std::vector<int> keepKind;
-          for (int i = 0; i < (int)leaves.size(); i++) if (!drop[i]) { keep.push_back(leaves[i]); keepKind.push_back(kinds[i]); }
-          leaves = std::move(keep); kinds = std::move(keepKind);
+        if (!lazyOfRoot_.count(t->index)) continue;
+        if (exactSums) {   // the other scalar-weighted leaves: taps of the first call, when they are computed before that call is issued
+          const auto [li, o] = lazyOfRoot_.at(t->index).front();
+          LazySum &L = lazy_[li];
+          for (int i = 0; i < (int)leaves.size(); i++) {
+            double v;
+            if (drop[i] || kinds[i] != 1 || vals_[leaves[i].first->index].size != 2 || !scalarWeight(leaves[i].second, v)) continue;
+            const Term *ct = leaves[i].first;
+            const bool rot0 = (ct->op == Op::RotateLeftConst || ct->op == Op::RotateRightConst) && *ct->rotation == 0;
+            const Term *src = rot0 ? C(ct->operandAt(0).get()) : ct;
+            if (vals_[src->index].fused || pos[src->index] >= pos[L.roots.front()->index]) continue;
+            if (v == 0.0) { drop[i] = 1; if (rot0) lazyUses[ct->index]++; continue; }
+            auto tp = std::find(L.taps.begin(), L.taps.end(), src);
+            if (tp == L.taps.end()) {
+              if (L.taps.size() >= 16) continue;
+              L.taps.push_back(src); for (auto &w : L.twts) w.push_back(nullptr); tp = L.taps.end() - 1;
+            }
+            auto &slot = L.twts[o][tp - L.taps.begin()];
+            if (slot) continue;
+            slot = leaves[i].second;
+            drop[i] = 1;
+            if (rot0) lazyUses[ct->index]++;   // read through its operand: the copy itself may never be made
+          }
         }
+        std::vector<std::pair<const Term *, const Term *>> keep; std::vector<int> keepKind;
+        for (int i = 0; i < (int)leaves.size(); i++) if (!drop[i]) { keep.push_back(leaves[i]); keepKind.push_back(kinds[i]); }
+        leaves = std::move(keep); kinds = std::move(keepKind);
+        if (exactSums && leaves.empty() && lazyOfRoot_.at(t->index).size() == 1) directOf_[t->index] = lazyOfRoot_.at(t->index).front();
       }
       for (auto &L : lazy_) { L.tempOff = arenaWords; arenaWords += L.roots.size() * 2 * (std::size_t)L.ell * N_; }
+      for (auto &kv : directOf_) vals_[kv.first].off = lazy_[kv.second.first].tempOff + (std::size_t)kv.second.second * 2 * lazy_[kv.second.first].ell * N_;
       for (auto &t : order_)
         if (lazyUses[t->index] && lazyUses[t->index] == usesAll[t->index]) vals_[t->index].fused = true;   // the rotation is never materialised
     }
@@ -559,11 +620,39 @@ private:
       streamOf[st.producer] = chosen;
       steps_.push_back(st);
     };
+    // the pseudo step of a rotation sum call, issued before the first fused sum it feeds
+    auto emitLazy = [&](int li) {
+      LazySum &Lz = lazy_[li];
+      const std::uint64_t lid = TC + hoistSrc.size() + (std::size_t)li;
+      if (Lz.emitted) return lid;
+      if (!hoistDone[Lz.gid]) {
+        Step hs;
+        hs.term = hoistSrc[Lz.gid]; hs.op = Op::Undef; hs.hoist = Lz.gid; hs.producer = TC + Lz.gid;
+        emit(hs, {hoistSrc[Lz.gid]->index}, -1, 0);
+        hoistDone[Lz.gid] = 1;
+      }
+      Step ls;
+      ls.term = hoistSrc[Lz.gid]; ls.op = Op::Undef; ls.lazy = li; ls.producer = lid;
+      std::vector<std::uint64_t> lops{hoistSrc[Lz.gid]->index, TC + (std::uint64_t)Lz.gid};
+      for (auto &ws : Lz.wts) for (const Term *w : ws) if (w && streamOf[w->index] >= 0) lops.push_back(w->index);   // (later sums' constants: same encode group)
+      for (auto &ws : Lz.twts) for (const Term *w : ws) if (w && streamOf[w->index] >= 0) lops.push_back(w->index);
+      for (const Term *x : Lz.taps) lops.push_back(x->index);
+      const std::size_t work = exactSums ? evab_rotate_wsum_work_bytes(dev_->ctx(), Lz.ell, (int)Lz.rots.size(), (int)Lz.roots.size())
+                                         : evab_lazy_rotsum_work_bytes(dev_->ctx(), Lz.ell, (int)Lz.roots.size());
+      emit(ls, lops, -1, work / 8);
+      Lz.emitted = true;
+      return lid;
+    };
     for (auto &t : order_) {
       const ValueInfo &v = vals_[t->index];
       const bool device = (v.kind == Kind::Cipher || v.kind == Kind::Plain) && t->op != Op::Input && !v.alias && !v.fused;
       if (!device) {
         if (v.alias) streamOf[t->index] = streamOf[aliasSource(t)];
+        continue;
+      }
+      if (auto d = directOf_.find(t->index); d != directOf_.end()) {   // the sum is a rotation sum call's output
+        const std::uint64_t lid = emitLazy(d->second.first);
+        prodOf[t->index] = lid; streamOf[t->index] = streamOf[lid];
         continue;
       }
       Step st;
@@ -573,23 +662,8 @@ private:
       for (const Term *o : stepOperands(t)) operands.push_back(o->index);
       if (auto lz = lazyOfRoot_.find(t->index); lz != lazyOfRoot_.end())
         for (auto &lo : lz->second) {   // the lazy rotation sums feeding this fused sum go first, as a pseudo step of their own
-          LazySum &Lz = lazy_[lo.first];
-          const std::uint64_t lid = TC + hoistSrc.size() + (std::size_t)lo.first;
-          if (!Lz.emitted) {
-            if (!hoistDone[Lz.gid]) {
-              Step hs;
-              hs.term = hoistSrc[Lz.gid]; hs.op = Op::Undef; hs.hoist = Lz.gid; hs.producer = TC + Lz.gid;
-              emit(hs, {hoistSrc[Lz.gid]->index}, -1, 0);
-              hoistDone[Lz.gid] = 1;
-            }
-            Step ls;
-            ls.term = hoistSrc[Lz.gid]; ls.op = Op::Undef; ls.lazy = lo.first; ls.producer = lid;
-            std::vector<std::uint64_t> lops{hoistSrc[Lz.gid]->index, TC + (std::uint64_t)Lz.gid};
-            for (auto &ws : Lz.wts) for (const Term *w : ws) if (w && streamOf[w->index] >= 0) lops.push_back(w->index);   // (later sums' constants: same encode group)
-            emit(ls, lops, -1, evab_lazy_rotsum_work_bytes(dev_->ctx(), Lz.ell, (int)Lz.roots.size()) / 8);
-            Lz.emitted = true;
-          }
-          st.lazyTemps.push_back(Lz.tempOff + (std::size_t)lo.second * 2 * Lz.ell * N_);
+          const std::uint64_t lid = emitLazy(lo.first);
+          st.lazyTemps.push_back(lazy_[lo.first].tempOff + (std::size_t)lo.second * 2 * lazy_[lo.first].ell * N_);
           operands.push_back(lid);
         }
       int forced = -1;
@@ -746,7 +820,9 @@ private:
     std::vector<int> bufOfVal(TC, -1), hoistBuf(H, -1), lazyBuf(L, -1), chunkBuf(chunks_.size(), -1), groupBuf(groups_.size(), -1);
     for (auto &t : order_) {
       const ValueInfo &v = vals_[t->index];
-      if ((v.kind != Kind::Cipher && v.kind != Kind::Plain) || v.alias || v.fused || t->op == Op::Encode || chunkOf_.count(t->index)) continue;
+      if ((v.kind != Kind::Cipher && v.kind != Kind::Plain) || v.alias || v.fused || t->op == Op::Encode || chunkOf_.count(t->index) ||
+          directOf_.count(t->index))
+        continue;
       const std::size_t words = (std::size_t)(v.kind == Kind::Cipher ? v.size : 1) * v.ell * N_;
       bufOfVal[t->index] = t->op == Op::Input ? newBuf(words, 0, true) : newBuf(words, stepOf.at(t->index), false);
     }
@@ -771,6 +847,7 @@ private:
       while (vals_[x].alias) x = aliasSource(byIndex_[x]);
       if (vals_[x].kind != Kind::Cipher && vals_[x].kind != Kind::Plain) return -1;
       if (auto c = chunkOf_.find(x); c != chunkOf_.end()) return chunkBuf[c->second];
+      if (auto d = directOf_.find(x); d != directOf_.end()) return lazyBuf[d->second.first];
       if (byIndex_[x]->op == Op::Encode) return groupBuf[groupIndex_.at(x)];
       return bufOfVal[x];
     };
@@ -784,6 +861,8 @@ private:
         if (st.lazy >= 0) {
           read(i, hoistBuf[lazy_[st.lazy].gid]);
           for (auto &ws : lazy_[st.lazy].wts) for (const Term *w : ws) if (w) read(i, bufOfTerm(w->index));
+          for (auto &ws : lazy_[st.lazy].twts) for (const Term *w : ws) if (w) read(i, bufOfTerm(w->index));
+          for (const Term *x : lazy_[st.lazy].taps) read(i, bufOfTerm(x->index));
         }
         continue;
       }
@@ -802,6 +881,7 @@ private:
         if (opt_.hoistModUp) hoistExtOff_[g] = hoistOff_[g] + (std::size_t)vals_[hoistSrc[g]->index].ell * N_;
       }
     for (std::size_t l = 0; l < L; l++) lazy_[l].tempOff = at(lazyBuf[l]);
+    for (auto &kv : directOf_) vals_[kv.first].off = lazy_[kv.second.first].tempOff + (std::size_t)kv.second.second * 2 * lazy_[kv.second.first].ell * N_;
     for (std::size_t c = 0; c < chunks_.size(); c++) {
       RotChunk &ch = chunks_[c];
       ch.outOff = at(chunkBuf[c]);
@@ -969,15 +1049,22 @@ private:
                                    keys.data(), cadds.data(), arena_.get() + workOff_[st.stream], stream));
       return;
     }
-    if (st.lazy >= 0) {   // approxHoist: out_o = sum_i w_oi (.) rotate(x, g_i), one mod-down per sum
+    if (st.lazy >= 0) {   // out_o = sum_i w_oi (.) rotate(x, g_i): approxHoist, one mod-down per sum; rotationSums, exact (+ taps)
       const LazySum &Lz = lazy_[st.lazy];
-      std::vector<u64> elts; std::vector<const u64 *> keys, cadds, wts;
+      std::vector<u64> elts; std::vector<const u64 *> keys, cadds, wts, taps, twts;
       for (const Term *r : Lz.rots) {
         const u64 elt = galoisElt(*r);
         elts.push_back(elt); keys.push_back(keys_.galois.at(elt).get());
         cadds.push_back(hoistConst_.at(std::make_pair(elt, Lz.ell)).get());
       }
       for (auto &ws : Lz.wts) for (const Term *w : ws) wts.push_back(w ? arena_.get() + vals_[w->index].off : nullptr);
+      if (!opt_.approxHoist) {
+        for (const Term *x : Lz.taps) taps.push_back(arena_.get() + vals_[x->index].off);
+        for (auto &ws : Lz.twts) for (const Term *w : ws) twts.push_back(w ? arena_.get() + vals_[w->index].off : nullptr);
+        check(evab_rotate_wsum(c, Lz.ell, (int)Lz.roots.size(), arena_.get() + Lz.tempOff, arena_.get() + o.off, arena_.get() + hoistExtOff_[Lz.gid], (int)elts.size(),
+                               elts.data(), keys.data(), cadds.data(), wts.data(), (int)taps.size(), taps.data(), twts.data(), arena_.get() + workOff_[st.stream], stream));
+        return;
+      }
       check(evab_lazy_rotsum(c, Lz.ell, (int)Lz.roots.size(), arena_.get() + Lz.tempOff, arena_.get() + o.off, arena_.get() + hoistExtOff_[Lz.gid], (int)elts.size(),
                              elts.data(), keys.data(), cadds.data(), wts.data(), arena_.get() + workOff_[st.stream], stream));
       return;
@@ -1097,6 +1184,7 @@ private:
   std::unordered_map<std::uint64_t, int> chunkOf_;
   std::vector<LazySum> lazy_;                                // approxHoist
   std::unordered_map<std::uint64_t, std::vector<std::pair<int, int>>> lazyOfRoot_;   // fused sum -> (lazy sum, output)
+  std::unordered_map<std::uint64_t, std::pair<int, int>> directOf_;   // rotationSums: fused sum stored as (lazy sum, output) itself
   std::set<std::uint64_t> needP_;                            // Encode terms whose plaintext carries the extra row mod P
   std::vector<std::size_t> hoistExtOff_;                     // ... and of the group's extended digits (hoistModUp)
   std::size_t flagsOff_ = 0, numFlags_ = 0;                  // zero-coefficient flags, 8 words apart

@@ -183,17 +183,18 @@ PYBIND11_MODULE(_eva_b200, m) {
              { py::gil_scoped_release rel; outs = p.collect(*h->batch); }
              return outs;
            }, py::arg("handle"))
-      .def("set_options", [](B200Public &p, int streams, bool graph, bool cache, bool dedup, int fuse, bool fuseSums, bool hoist, bool uniformEncode, bool dedupTerms, bool hoistModUp, bool approxHoist, int rotationChunk, std::size_t arenaLimit) {
+      .def("set_options", [](B200Public &p, int streams, bool graph, bool cache, bool dedup, int fuse, bool fuseSums, bool hoist, bool uniformEncode, bool dedupTerms, bool hoistModUp, bool approxHoist, int rotationChunk, std::size_t arenaLimit, bool rotationSums) {
              p.options.numStreams = streams; p.options.useGraph = graph; p.options.cacheConstants = cache; p.options.dedupConstants = dedup;
              p.options.fuse = fuse; p.options.fuseSums = fuseSums; p.options.hoistRotations = hoist; p.options.uniformEncode = uniformEncode;
              p.options.dedupTerms = dedupTerms; p.options.hoistModUp = hoistModUp; p.options.approxHoist = approxHoist; p.options.rotationChunk = rotationChunk;
-             p.options.arenaLimit = arenaLimit;
+             p.options.arenaLimit = arenaLimit; p.options.rotationSums = rotationSums;
            },
            py::arg("num_streams") = 8, py::arg("use_graph") = true, py::arg("cache_constants") = true, py::arg("dedup_constants") = true,
            py::arg("fuse") = 1, py::arg("fuse_sums") = true, py::arg("hoist_rotations") = true, py::arg("uniform_encode") = true, py::arg("dedup_terms") = true, py::arg("hoist_mod_up") = true, py::arg("approx_hoist") = false, py::arg("rotation_chunk") = 16,
-           py::arg("arena_limit") = 0,
+           py::arg("arena_limit") = 0, py::arg("rotation_sums") = true,
            "arena_limit: bytes one plan's arena may take (0: the free device memory when the plan is built).  A plan whose one-offset-per-value "
-           "layout does not fit reuses the storage of dead values; if even that exceeds the limit, building the plan raises RuntimeError")
+           "layout does not fit reuses the storage of dead values; if even that exceeds the limit, building the plan raises RuntimeError.  "
+           "rotation_sums: sums of rotations of one ciphertext weighted by scalar constants run as one bit-exact evab_rotate_wsum call (approx_hoist takes precedence)")
       .def("set_input_sizes", [](B200Public &p, const std::map<std::string, int> &sizes) { p.options.inputSizes = sizes; },
            "ciphertext inputs that are not size 2 (name -> polynomials); applies to plans built afterwards")
       .def("drop_plan", &B200Public::dropExecutor, py::arg("program"), py::arg("batch") = 1, py::arg("replica") = 0)

@@ -115,17 +115,23 @@ template <class BE> int mulct_impl(BE &be, const CtxView &c, bool square, int el
 // rescale and the key-switch mod-down.  Poly q (< npoly) of `in` has `nres`
 // residues: prime indices pm[0..nres-2] followed by the divisor `last`.
 //   out[q][r] = (in[q][r] - NTT((iNTT(in[q][last]) + h) mod q_last mod q_r - h mod q_r)) * q_last^-1  (+ add[q][r])
+// first half: tmp[q] = iNTT(in[q][last]) + h, canonical mod q_last
 template <class BE>
-int divround_impl(BE &be, const CtxView &c, const u64 *in, long long in_poly_stride, int npoly, int nres, const unsigned char *pm,
-                  int last, u64 *out, long long out_poly_stride, const u64 *add, long long add_poly_stride, u64 *tmp,
-                  int add_polys = 1 << 30, const u32 *add_perm = nullptr) {
+int divround_inv_impl(BE &be, const CtxView &c, const u64 *in, long long in_poly_stride, int npoly, int nres, int last, u64 *tmp) {
   const long long N = (long long)c.N;
   NttLaunch A = base_launch(c);
   A.src = in + (long long)(nres - 1) * N; A.dst = tmp;
   A.src_sq = in_poly_stride; A.dst_sq = N; A.inner = 1; A.prime_on_q = 1;
   for (int q = 0; q < npoly; q++) A.pmap[q] = (unsigned char)last;
   A.epi = EPI_ADDHALF;
-  if (int rc = be.inv(A, npoly)) return rc;
+  return be.inv(A, npoly);
+}
+template <class BE>
+int divround_impl(BE &be, const CtxView &c, const u64 *in, long long in_poly_stride, int npoly, int nres, const unsigned char *pm,
+                  int last, u64 *out, long long out_poly_stride, const u64 *add, long long add_poly_stride, u64 *tmp,
+                  int add_polys = 1 << 30, const u32 *add_perm = nullptr) {
+  const long long N = (long long)c.N;
+  if (int rc = divround_inv_impl(be, c, in, in_poly_stride, npoly, nres, last, tmp)) return rc;
   NttLaunch B = base_launch(c);
   B.src = tmp; B.src_sq = N; B.src_sr = 0;
   B.aux0 = in; B.aux0_sq = in_poly_stride; B.aux0_sr = N;
@@ -342,6 +348,54 @@ int rotate_modup_many_impl(BE &be, const CtxView &c, int ell, int n, u64 *out, c
   unsigned char pm[32];
   for (int i = 0; i < ell; i++) pm[i] = (unsigned char)i;
   return divround_impl(be, c, acc, (long long)(ell + 1) * N, 2 * n, ell + 1, pm, c.k - 1, out, (long long)ell * N, (const u64 *)nullptr, 0, tmp);
+}
+
+// ---- rotate_wsum: out_o = sum_i w_oi (.) rotate(a, g_i) + sum_t w_ot (.) taps[t], every w a scalar plaintext [ell][N] (null: 0), in
+// four launches: the inner products of rotate_modup_many_impl, the inverse NTT of their 2n P rows, the weighting (k_rot_wsum, see
+// WsumArgs) and the forward NTT + division of the 2 nout ell weighted rows.  Same bits as rotate -> multiply_plain -> add: the
+// forward NTT is linear, so it commutes with the weighting, and every rotation keeps its own rounding by P.  n(2 + 2 ell)
+// transforms become 2n + 2 nout ell.  taps: size-2 ciphertexts at level ell (plain multiply_plain leaves of the sums).
+// out [nout][2][ell][N]; wts[o*n+i], twts[o*ntap+t]; work: rotate_wsum_work_elems.
+inline size_t rotate_wsum_work_elems(const CtxView &c, int ell, int n, int nout) {
+  return rotate_modup_many_work_elems(c, ell, n) + (size_t)2 * nout * 2 * ell * c.N;
+}
+template <class BE>
+int rotate_wsum_impl(BE &be, const CtxView &c, int ell, int nout, u64 *out, const u64 *a, const u64 *ext, int n, const u32 *const *perms,
+                     const u64 *const *keys, const u64 *const *cadds, const u64 *const *wts, int ntap, const u64 *const *taps,
+                     const u64 *const *twts, u64 *work) {
+  if (ell < 1 || ell > c.k - 1) return be.error("rotate_wsum needs 1 <= ell <= k-1");
+  if (n < 1 || n > WS_MAX) return be.error("rotate_wsum: 1..16 rotations");
+  if (nout < 1 || nout > WS_OUT) return be.error("rotate_wsum: 1..4 output sums");
+  if (ntap < 0 || ntap > WS_TAPS) return be.error("rotate_wsum: 0..16 plain taps");
+  const long long N = (long long)c.N;
+  u64 *acc = work, *tmp = acc + (size_t)n * 2 * (ell + 1) * N;
+  u64 *A = tmp + (size_t)n * 2 * N, *D = A + (size_t)nout * 2 * ell * N;
+  RotManyArgs R;
+  memset(&R, 0, sizeof(R));
+  R.t = a + (size_t)ell * N; R.ext = ext; R.acc = acc; R.primes = c.primes; R.n = n; R.ell = ell; R.k = c.k; R.N = (int)N;
+  for (int i = 0; i < n; i++) { R.perm[i] = perms[i]; R.key[i] = keys[i]; R.cadd[i] = cadds[i]; }
+  if (int rc = be.rot_many(R)) return rc;
+  if (int rc = divround_inv_impl(be, c, acc, (long long)(ell + 1) * N, 2 * n, ell + 1, c.k - 1, tmp)) return rc;
+  WsumArgs W;
+  memset(&W, 0, sizeof(W));
+  W.acc = acc; W.tmp = tmp; W.A = A; W.D = D; W.primes = c.primes; W.halfmod = c.halfmod + (size_t)(c.k - 1) * c.k;
+  W.n = n; W.ntap = ntap; W.nout = nout; W.ell = ell; W.k = c.k; W.N = (int)N;
+  for (int o = 0; o < nout; o++) {
+    for (int i = 0; i < n; i++) W.wt[o][i] = wts[(size_t)o * n + i];
+    for (int t = 0; t < ntap; t++) W.twt[o][t] = twts[(size_t)o * ntap + t];
+  }
+  for (int t = 0; t < ntap; t++) W.tap[t] = taps[t];
+  if (int rc = be.rot_wsum(W)) return rc;
+  NttLaunch B = base_launch(c);
+  B.src = D; B.src_sq = ell * N; B.src_sr = N;
+  B.aux0 = A; B.aux0_sq = ell * N; B.aux0_sr = N;
+  B.dst = out; B.dst_sq = ell * N; B.dst_sr = N;
+  B.inner = ell; B.prime_on_q = 0;
+  for (int r = 0; r < ell; r++) { B.pmap[r] = (unsigned char)r; B.pmap2[r] = (unsigned char)(c.k - 1); }
+  B.pro = PRO_PLAIN; B.epi = EPI_DIVROUND;
+  B.consts = c.qinv + (size_t)(c.k - 1) * c.k;
+  B.consts_f = c.qinv_f + (size_t)(c.k - 1) * c.k;
+  return be.fwd(B, (size_t)nout * 2 * ell);
 }
 
 // seal::CKKSEncoder::encode (vector overload) for a batch of vectors -- reference

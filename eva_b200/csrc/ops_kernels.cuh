@@ -281,6 +281,73 @@ EVAB_HD void hoist_const_elem(const HoistConstArgs &A, int mi, int j) {
 // I_g as residues: row mi, coefficient j = sign bit of the coefficient-domain gather table
 EVAB_HD void hoist_indicator_elem(u64 *out, const u32 *ctab, int N, int mi, int j) { out[(size_t)mi * N + j] = EVAB_LDG(ctab + j) & 1u; }
 
+// ---- rotate_wsum (exact): sums of rotations of one ciphertext weighted by scalar plaintexts (ops_impl.hpp rotate_wsum_impl).
+// A scalar weight is a constant polynomial: in the NTT domain one number w_r per residue, read at pt[r * N].  With acc_i the
+// key-switch accumulator of rotation i and tmp_i = iNTT_P(acc_i's P row) + floor(P/2), every output word is
+//   A[o][c][r] = sum_i w_oir acc_i[c][r] + sum_t (P mod q_r) w_otr x_t[c][r]     (folded plain taps: divided by P they give w x_t)
+//   D[o][c][r] = sum_i w_oir ((tmp_i[c] mod q_r) - floor(P/2) mod q_r)
+// and the forward NTT of D with the division epilogue (A - NTT(D)) P^-1 gives sum_i w_oi rotate(x, g_i) + sum_t w_ot x_t, the
+// rounding of every rotation being its own.  Products are accumulated in 128 bits and reduced once per output word: tmp_i < P
+// enters unreduced, and -floor(P/2) as + (q_r - floor(P/2) mod q_r), the same residue as pro_load's MODRED; every product is
+// below 2^121 (primes < 2^60), so the WS_MAX + WS_TAPS products of one output word fit.
+#define WS_MAX 16
+#define WS_TAPS 16
+#define WS_OUT 4
+struct WsumArgs {
+  const u64 *acc;                  // [n][2][ell+1][N] (k_rot_many)
+  const u64 *tmp;                  // [n][2][N]        (inverse NTT of the P rows, + floor(P/2))
+  const u64 *wt[WS_OUT][WS_MAX];   // scalar plaintexts [ell][N] (batch instance offset applies); null: weight 0
+  const u64 *tap[WS_TAPS];         // size-2 ciphertexts [2][ell][N] at the output's level (batch instance offset applies)
+  const u64 *twt[WS_OUT][WS_TAPS]; // their scalar weights; null: weight 0
+  u64 *A, *D;                      // [nout][2][ell][N]
+  const PrimeDev *primes;
+  const u64 *halfmod;              // [k]: floor(P/2) mod q_r
+  int n, ntap, nout, ell, k, N;
+};
+// coefficients j, j+1 of residue r of polynomial c of every output
+EVAB_HD void rot_wsum_elem(const WsumArgs &A, int c, int r, int j, long long off = 0) {
+  const PrimeDev P = A.primes[r];
+  const size_t N = A.N;
+  const u64 nh = P.p - A.halfmod[r];
+  u64 al[WS_OUT][2], ah[WS_OUT][2], dl[WS_OUT][2], dh[WS_OUT][2];
+#pragma unroll
+  for (int o = 0; o < WS_OUT; o++) al[o][0] = al[o][1] = ah[o][0] = ah[o][1] = dl[o][0] = dl[o][1] = dh[o][0] = dh[o][1] = 0;
+  for (int i = 0; i < A.n; i++) {
+    const u64x2 a = ld2(A.acc + off + (((size_t)i * 2 + c) * (A.ell + 1) + r) * N + j);
+    u64x2 t = ld2(A.tmp + off + ((size_t)i * 2 + c) * N + j);
+    t.x += nh; t.y += nh;
+#pragma unroll
+    for (int o = 0; o < WS_OUT; o++) {
+      if (o >= A.nout || !A.wt[o][i]) continue;
+      const u64 w = EVAB_LDG(A.wt[o][i] + off + (size_t)r * N);
+      mac128(al[o][0], ah[o][0], a.x, w); mac128(al[o][1], ah[o][1], a.y, w);
+      mac128(dl[o][0], dh[o][0], t.x, w); mac128(dl[o][1], dh[o][1], t.y, w);
+    }
+  }
+  if (A.ntap) {
+    const u64 pm = barrett64(A.primes[A.k - 1].p, P.p, P.ratio64);   // P mod q_r
+    for (int t = 0; t < A.ntap; t++) {
+      const u64x2 x = ld2(A.tap[t] + off + ((size_t)c * A.ell + r) * N + j);
+#pragma unroll
+      for (int o = 0; o < WS_OUT; o++) {
+        if (o >= A.nout || !A.twt[o][t]) continue;
+        const u64 w = mulmod_p(pm, EVAB_LDG(A.twt[o][t] + off + (size_t)r * N), P);
+        mac128(al[o][0], ah[o][0], x.x, w); mac128(al[o][1], ah[o][1], x.y, w);
+      }
+    }
+  }
+#pragma unroll
+  for (int o = 0; o < WS_OUT; o++) {
+    if (o >= A.nout) break;
+    const size_t w = off + (((size_t)o * 2 + c) * A.ell + r) * N + j;
+    u64x2 v;
+    v.x = reduce128(al[o][0], ah[o][0], P); v.y = reduce128(al[o][1], ah[o][1], P);
+    st2(A.A + w, v);
+    v.x = reduce128(dl[o][0], dh[o][0], P); v.y = reduce128(dl[o][1], dh[o][1], P);
+    st2(A.D + w, v);
+  }
+}
+
 // ---- lazy_rotsum (OPT-IN, NOT bit-exact: SURVEY 8f-4) ------------------------------------------------------------------
 // sum_i w_i (.) rotate(x, g_i) for several rotations of ONE ciphertext with plaintext weights, with a single mod-down for the
 // whole sum: T[c][m] = sum_i w_i[m] (.) acc_i[c][m] over the extended basis (q_0 .. q_{ell-1}, P), acc_i the key-switch

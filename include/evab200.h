@@ -197,12 +197,22 @@ int evab_rotate_modup_prepared(evab_ctx *ctx, int ell, uint64_t *d_out, const ui
                                const uint64_t *d_key, const uint64_t *d_cadd, void *d_work, void *stream);
 /* n <= 16 rotations of ONE ciphertext (seal::Evaluator::rotate_vector, seal_executor.h:176-189) in three kernel launches instead of
  * 3 n: d_out [n][2][ell][N], rotation i by galois_elts[i]; same bits as n calls of evab_rotate_modup_prepared.  d_ext, keys, cadds as there. */
-/* evab_rotate_modup_many and evab_lazy_rotsum read P * c0 from the diagonal of d_ext (ext[m][J] has no entry for m = q_J): call this once
+/* evab_rotate_modup_many, evab_rotate_wsum and evab_lazy_rotsum read P * c0 from the diagonal of d_ext (ext[m][J] has no entry for m = q_J): call this once
  * per ciphertext after evab_rotate_modup_prepare and before either of them. */
 int evab_rotate_modup_scale_c0(evab_ctx *ctx, int ell, uint64_t *d_ext, const uint64_t *d_a, void *stream);
 size_t evab_rotate_modup_many_work_bytes(const evab_ctx *ctx, int ell, int n);
 int evab_rotate_modup_many(evab_ctx *ctx, int ell, int n, uint64_t *d_out, const uint64_t *d_a, const uint64_t *d_ext, const uint64_t *galois_elts,
                            const uint64_t *const *d_keys, const uint64_t *const *d_cadds, void *d_work, void *stream);
+/* Bit-exact weighted rotation sums: d_out [nout][2][ell][N], out_o = sum_i w_oi (.) rotate(x, g_i) + sum_t v_ot (.) c_t for n <= 16
+ * rotations of ONE ciphertext x = d_a, nout <= 4 sums and ntap <= 16 size-2 ciphertexts c_t = d_taps[t] at level ell; the same bits as
+ * rotate -> multiply_plain -> add (every rotation keeps its own rounding by P), in four launches and 2 n + 2 nout ell transforms instead of
+ * n (2 + 2 ell).  Every weight is a SCALAR plaintext [ell][N] (the encoding of a replicated constant: one value per residue);
+ * d_wts[o * n + i] weighs rotation i in sum o, d_twts[o * ntap + t] tap t, NULL for weight 0.  d_ext, keys, cadds as for
+ * evab_rotate_modup_many (after evab_rotate_modup_scale_c0). */
+size_t evab_rotate_wsum_work_bytes(const evab_ctx *ctx, int ell, int n, int nout);
+int evab_rotate_wsum(evab_ctx *ctx, int ell, int nout, uint64_t *d_out, const uint64_t *d_a, const uint64_t *d_ext, int n, const uint64_t *galois_elts,
+                     const uint64_t *const *d_keys, const uint64_t *const *d_cadds, const uint64_t *const *d_wts, int ntap,
+                     const uint64_t *const *d_taps, const uint64_t *const *d_twts, void *d_work, void *stream);
 /* OPT-IN, NOT bit-exact (SURVEY 8f-4; graded by the reference's MSE criterion only): d_out [nout][2][ell][N],
  * out_o = sum_i w_oi (.) rotate(x, g_i) for n <= 16 rotations of ONE ciphertext x = d_a and nout <= 4 sets of plaintext weights, rounding
  * each weighted sum down by P ONCE instead of every rotation (2 + 2 ell transforms per sum instead of n (2 + 2 ell)); the key-switch
