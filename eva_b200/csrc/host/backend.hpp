@@ -136,7 +136,7 @@ public:
       ExecOptions o = options;
       o.batch = batch;
       h->opt = o;   // as requested (what the staleness test above compares)
-      h->exec = std::make_unique<Executor>(s_->dev, s_->client->encoder(), s_->keys, program, o);
+      h->exec = std::make_unique<Executor>(s_->dev, s_->keys, program, o);
       h->termCount = program.termCount();
       program.attach(key, h);
     }

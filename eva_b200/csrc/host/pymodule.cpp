@@ -26,6 +26,29 @@ static void requireShape(const u64arr &a, std::initializer_list<std::size_t> sha
   if (!ok) throw std::runtime_error(std::string(what) + " does not match the parameters (modulus count / degree)");
 }
 
+// set_options: one argument list for B200Public and for the planner test hook (_plan), which parses its options dict through it
+static ExecOptions &optionsOf(B200Public &p) { return p.options; }
+static ExecOptions &optionsOf(ExecOptions &o) { return o; }
+template <class Self>
+static void setOptions(Self &self, int streams, bool graph, bool cache, bool dedup, int fuse, bool fuseSums, bool hoist, bool uniformEncode, bool dedupTerms,
+                       bool hoistModUp, bool approxHoist, int rotationChunk, std::size_t arenaLimit, bool rotationSums) {
+  ExecOptions &o = optionsOf(self);
+  o.numStreams = streams; o.useGraph = graph; o.cacheConstants = cache; o.dedupConstants = dedup;
+  o.fuse = fuse; o.fuseSums = fuseSums; o.hoistRotations = hoist; o.uniformEncode = uniformEncode;
+  o.dedupTerms = dedupTerms; o.hoistModUp = hoistModUp; o.approxHoist = approxHoist; o.rotationChunk = rotationChunk;
+  o.arenaLimit = arenaLimit; o.rotationSums = rotationSums;
+}
+template <class Class>
+static void defSetOptions(Class &cls) {
+  cls.def("set_options", &setOptions<typename Class::type>,
+          py::arg("num_streams") = 8, py::arg("use_graph") = true, py::arg("cache_constants") = true, py::arg("dedup_constants") = true,
+          py::arg("fuse") = 1, py::arg("fuse_sums") = true, py::arg("hoist_rotations") = true, py::arg("uniform_encode") = true, py::arg("dedup_terms") = true, py::arg("hoist_mod_up") = true, py::arg("approx_hoist") = false, py::arg("rotation_chunk") = 16,
+          py::arg("arena_limit") = 0, py::arg("rotation_sums") = true,
+          "arena_limit: bytes one plan's arena may take (0: the free device memory when the plan is built).  A plan whose one-offset-per-value "
+          "layout does not fit reuses the storage of dead values; if even that exceeds the limit, building the plan raises RuntimeError.  "
+          "rotation_sums: sums of rotations of one ciphertext weighted by scalar constants run as one bit-exact evab_rotate_wsum call (approx_hoist takes precedence)");
+}
+
 // execute_batch_async handle: the batch plus the Python objects it reads from.  Destroyed with the GIL held (the batch first:
 // it waits for its copies before the valuations may go)
 struct PyPending {
@@ -102,6 +125,39 @@ PYBIND11_MODULE(_eva_b200, m) {
     PackResult r = packArena(ps, pb);
     return py::make_tuple(r.offsets, r.waits, r.peak);
   }, py::arg("steps"), py::arg("buffers"));
+  // test hook: the planner alone (host/planner.hpp), without a device.  options: set_options' keywords; arena_limit 0 is no limit
+  // here.  The scratch sizes are stand-ins derived from N and ell (the layout's invariants hold for any sizes)
+  py::class_<ExecOptions> planOptions(m, "_PlanOptions");
+  planOptions.def(py::init<>());
+  defSetOptions(planOptions);
+  m.def("_plan", [](Program &prog, std::uint64_t N, int k, const py::dict &options, int batch) {
+    py::object holder = py::cast(ExecOptions{});
+    holder.attr("set_options")(**options);
+    ExecOptions opt = holder.cast<ExecOptions>();
+    opt.batch = batch;
+    WorkSizes ws;
+    ws.keyswitch = ws.rotateModupExt = [N](int ell) { return (std::size_t)(ell + 1) * ell * N * 8; };
+    ws.rescale = [N](int size) { return (std::size_t)size * N * 8; };
+    ws.rotateModupMany = [N](int ell, int n) { return (std::size_t)n * (ell + 1) * N * 8; };
+    ws.rotateWsum = [N](int ell, int n, int nout) { return (std::size_t)(n + nout) * (ell + 1) * N * 8; };
+    ws.lazyRotsum = [N](int ell, int nout) { return (std::size_t)nout * (ell + 1) * N * 8; };
+    ws.encode = [N](int count) { return (std::size_t)count * N * 16; };
+    const Plan p = buildPlan(prog, opt, N, k, opt.arenaLimit ? opt.arenaLimit : SIZE_MAX, ws);
+    static const char *kinds[] = {"Term", "Hoist", "RotationChunk", "RotationSum"};
+    py::list steps, regions;
+    for (auto &st : p.steps) steps.append(py::make_tuple(kinds[(int)st.kind], st.term->index, st.stream, st.waits, st.record));
+    for (auto &r : p.regions) regions.append(py::make_tuple(p.laidWords(r), r.off, r.writer, r.readers, r.pinned));
+    py::dict values;   // materialised values: (offset, words, region)
+    for (auto &t : p.order)
+      if (int r = p.storage[t->index]; r >= 0) {
+        const ValueInfo &v = p.vals[t->index];
+        const std::size_t rows = v.kind == Kind::Cipher ? (std::size_t)v.size * v.ell : v.ell + (t->op == Op::Encode && p.groups[p.groupIndex.at(t->index)].withP);
+        values[py::int_(t->index)] = py::make_tuple(v.off, rows * N, r);
+      }
+    py::dict d;
+    d["steps"] = steps; d["regions"] = regions; d["values"] = values; d["stride"] = p.stride; d["stats"] = p.planStats();
+    return d;
+  }, py::arg("program"), py::arg("N"), py::arg("k"), py::arg("options") = py::dict(), py::arg("batch") = 1);
   m.def("set_num_threads", [](int) {}, py::arg("num_threads"),
         "Kept for API compatibility: the DAG is scheduled on CUDA streams, not CPU threads.");
   py::class_<int>(m, "_GaloisGuard").def(py::init());
@@ -160,8 +216,8 @@ PYBIND11_MODULE(_eva_b200, m) {
       });
 
   py::class_<PyPending, std::shared_ptr<PyPending>>(mb, "PendingBatch", "a submitted, not yet collected execute_batch");
-  py::class_<B200Public>(mb, "B200Public", "The public part of the context: encryption and execution on the GPU")
-      .def("encrypt", &B200Public::encrypt, py::arg("inputs"), py::arg("signature"))
+  py::class_<B200Public> pub(mb, "B200Public", "The public part of the context: encryption and execution on the GPU");
+  pub.def("encrypt", &B200Public::encrypt, py::arg("inputs"), py::arg("signature"))
       .def("execute", &B200Public::execute, py::arg("program"), py::arg("inputs"), py::call_guard<py::gil_scoped_release>())
       // the list is converted to pointers to the caller's valuations: no copy of the host ciphertexts
       .def("execute_batch", [](B200Public &p, Program &prog, const std::vector<const B200Valuation *> &in) { return p.executeMany(prog, in); },
@@ -183,18 +239,6 @@ PYBIND11_MODULE(_eva_b200, m) {
              { py::gil_scoped_release rel; outs = p.collect(*h->batch); }
              return outs;
            }, py::arg("handle"))
-      .def("set_options", [](B200Public &p, int streams, bool graph, bool cache, bool dedup, int fuse, bool fuseSums, bool hoist, bool uniformEncode, bool dedupTerms, bool hoistModUp, bool approxHoist, int rotationChunk, std::size_t arenaLimit, bool rotationSums) {
-             p.options.numStreams = streams; p.options.useGraph = graph; p.options.cacheConstants = cache; p.options.dedupConstants = dedup;
-             p.options.fuse = fuse; p.options.fuseSums = fuseSums; p.options.hoistRotations = hoist; p.options.uniformEncode = uniformEncode;
-             p.options.dedupTerms = dedupTerms; p.options.hoistModUp = hoistModUp; p.options.approxHoist = approxHoist; p.options.rotationChunk = rotationChunk;
-             p.options.arenaLimit = arenaLimit; p.options.rotationSums = rotationSums;
-           },
-           py::arg("num_streams") = 8, py::arg("use_graph") = true, py::arg("cache_constants") = true, py::arg("dedup_constants") = true,
-           py::arg("fuse") = 1, py::arg("fuse_sums") = true, py::arg("hoist_rotations") = true, py::arg("uniform_encode") = true, py::arg("dedup_terms") = true, py::arg("hoist_mod_up") = true, py::arg("approx_hoist") = false, py::arg("rotation_chunk") = 16,
-           py::arg("arena_limit") = 0, py::arg("rotation_sums") = true,
-           "arena_limit: bytes one plan's arena may take (0: the free device memory when the plan is built).  A plan whose one-offset-per-value "
-           "layout does not fit reuses the storage of dead values; if even that exceeds the limit, building the plan raises RuntimeError.  "
-           "rotation_sums: sums of rotations of one ciphertext weighted by scalar constants run as one bit-exact evab_rotate_wsum call (approx_hoist takes precedence)")
       .def("set_input_sizes", [](B200Public &p, const std::map<std::string, int> &sizes) { p.options.inputSizes = sizes; },
            "ciphertext inputs that are not size 2 (name -> polynomials); applies to plans built afterwards")
       .def("drop_plan", &B200Public::dropExecutor, py::arg("program"), py::arg("batch") = 1, py::arg("replica") = 0)
@@ -326,7 +370,8 @@ PYBIND11_MODULE(_eva_b200, m) {
         dev->upload(d.get(), pt.data(), pt.size() * 8);
         return p.shared()->client->encoder().decode(d.get(), (int)pt.shape(0), scale);
       });
-  py::class_<B200Secret>(mb, "B200Secret", "The secret part of the context: decryption")
+  defSetOptions(pub);
+  py::class_<B200Secret>(mb, "B200Secret","The secret part of the context: decryption")
       .def("decrypt", &B200Secret::decrypt, py::arg("enc_outputs"), py::arg("signature"))
       // test hook: Decryptor::decrypt of a raw ciphertext [size][ell][N] -> plaintext polynomial [ell][N] (before decoding)
       .def("decrypt_poly", [](B200Secret &x, const u64arr &ct) {

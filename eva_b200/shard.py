@@ -21,7 +21,7 @@ _ATTR_COPY = ("RescaleDivisorAttribute", "RangeAttribute", "EncodeAtScaleAttribu
 
 
 class Info:
-    """static value information of a compiled term (the rules of Executor::buildPlan / seal_executor.h)"""
+    """static value information of a compiled term (the rules of the planner's value inference, planner.hpp / seal_executor.h)"""
     __slots__ = ("type", "size", "level", "scale")
 
     def __init__(self, type_, size, level, scale):
