@@ -35,7 +35,7 @@ struct EncBatch {
   const cplx *roots;                  // [N] zeta^bitrev(i)
   const u32 *slot_index;              // [N]
   const PrimeDev *primes;
-  const u64 *pow2;                    // [k][128]: 2^i mod p
+  const u64 *pow2;                    // [k][ENC_POW2_ROW]: 2^i mod p
   u32 N, ell, count;
   u32 special_row;                    // != 0: the LAST of the ell rows is the residue mod prime `special_row` (the key-switch
                                       // prime P: plaintexts that multiply un-modded-down key-switch accumulators, lazy_rotsum)
@@ -92,8 +92,8 @@ EVAB_HD void enc_fft8(const EncBatch &B, u32 e, u32 t, u32 g, int nstages, long 
   else { for (u32 s = 0; s < 4; s++) enc_fft_set<1>(B, e, 4 * t + s, g, off); }
 }
 
-// rounded coefficient c (an integer-valued double of any magnitude) -> residue mod prime i
-// (sign-aware; exact beyond 2^64 through mantissa * 2^shift)
+// rounded coefficient c (an integer-valued double of any finite magnitude) -> residue mod prime i
+// (sign-aware; exact beyond 2^64 through mantissa * 2^shift, 1 <= shift <= 960 < ENC_POW2_ROW)
 EVAB_HD u64 enc_residue(double c, const PrimeDev &P, const u64 *pow2_row) {
   const bool neg = signbit(c);
   const double mag = fabs(c);
@@ -101,7 +101,8 @@ EVAB_HD u64 enc_residue(double c, const PrimeDev &P, const u64 *pow2_row) {
   if (mag < 18446744073709551616.0) mant = (u64)mag;
   else { int ex; const double fr = frexp(mag, &ex); mant = (u64)ldexp(fr, 64); sh = ex - 64; }
   u64 v = barrett64(mant, P.p, P.ratio64);
-  if (sh) v = mulmod(v, pow2_row[sh > 127 ? 127 : sh], P.p, P.ratio_lo, P.ratio_hi);
+  // the mask is the identity for every finite c; it only keeps a non-finite input's read inside the row
+  if (sh) v = mulmod(v, pow2_row[sh & (ENC_POW2_ROW - 1)], P.p, P.ratio_lo, P.ratio_hi);
   return (neg && v) ? P.p - v : v;
 }
 // coefficient j: round(re * scale / N) -> residue mod every prime
@@ -111,7 +112,7 @@ EVAB_HD void enc_round(const EncBatch &B, u32 e, u32 j, long long off = 0) {
   if (j > 0 && c != 0.0) (B.flags + off)[e] = 1;
   for (u32 i = 0; i < B.ell; i++) {
     const u32 pi = enc_prime_of_row(i, B.ell, B.special_row);
-    (B.out + off)[((size_t)e * B.ell + i) * B.N + j] = enc_residue(c, B.primes[pi], B.pow2 + (size_t)pi * 128);
+    (B.out + off)[((size_t)e * B.ell + i) * B.N + j] = enc_residue(c, B.primes[pi], B.pow2 + (size_t)pi * ENC_POW2_ROW);
   }
 }
 
@@ -133,7 +134,7 @@ EVAB_HD void enc_uniform_elem(const EncUniform &B, u32 e, u32 i, u32 j, long lon
   const double re = D_MUL(B.value[e], (double)B.N);            // log2(N) exact doublings of the FFT
   const double c = round(D_MUL(re, B.scale[e] / (double)B.N));
   const u32 pi = enc_prime_of_row(i, B.ell, B.special_row);
-  const u64 r = enc_residue(c, B.primes[pi], B.pow2 + (size_t)pi * 128);
+  const u64 r = enc_residue(c, B.primes[pi], B.pow2 + (size_t)pi * ENC_POW2_ROW);
   u64x2 v; v.x = r; v.y = r;
   *reinterpret_cast<u64x2 *>(B.out + off + ((size_t)e * B.ell + i) * B.N + j) = v;
 }

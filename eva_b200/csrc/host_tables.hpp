@@ -47,7 +47,7 @@ inline void unit_root(u64 index, u64 degree, double &re, double &im) {
 struct Tables {
   std::vector<cplxh> roots;        // [N] zeta^bitrev(i), zeta = e^(2 pi i / 2N)   (CKKS encoder)
   std::vector<u32> slot_index;     // [N] matrix_reps_index_map
-  std::vector<u64> pow2;           // [k][128] 2^i mod p
+  std::vector<u64> pow2;           // [k][ENC_POW2_ROW] 2^i mod p
   std::vector<u64x2> tw;       // [k][2][N]  forward / inverse {w, shoup(w)} in bit-reversed power order,
                                // followed by [k][2][N] {w, w * 2^32 mod p} (fold rows; zero for primes that are not fold-friendly)
   std::vector<PrimeDev> pd;    // tw / itw pointers are filled relative to `tw_base`
@@ -106,8 +106,11 @@ inline const char *build_tables(u64 N, int logN, const u64 *primes, int k, const
       T.slot_index[slots | i] = bitrev((u32)((m - pos - 1) >> 1), logN);
       pos = (pos * 3) & (m - 1);
     } }
-  T.pow2.assign((size_t)k * 128, 0);
-  for (int i = 0; i < k; i++) { u64 v = 1 % primes[i]; for (int e = 0; e < 128; e++) { T.pow2[(size_t)i * 128 + e] = v; v = mulmod(v, 2, primes[i]); } }
+  T.pow2.assign((size_t)k * ENC_POW2_ROW, 0);
+  for (int i = 0; i < k; i++) {
+    u64 v = 1 % primes[i];
+    for (int e = 0; e < ENC_POW2_ROW; e++) { T.pow2[(size_t)i * ENC_POW2_ROW + e] = v; v = mulmod(v, 2, primes[i]); }
+  }
   T.qinv.assign((size_t)k * k, u64x2{0, 0});
   T.qinv_f.assign((size_t)k * k, u64x2{0, 0});
   T.halfmod.assign((size_t)k * k, 0);

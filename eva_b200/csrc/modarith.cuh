@@ -53,6 +53,9 @@ struct FoldPrime {
   u64 ninv, ninv_v, itw1n, itw1n_v;
 };
 constexpr int NTT_MAX_PRIMES = 24;
+// entries per prime of the encoder's table 2^i mod p (host_tables.hpp, encode_kernels.cuh enc_residue): a finite double
+// c >= 2^64 is mant * 2^sh with sh = exponent - 64 <= 1024 - 64 = 960, so every shift has its row entry
+constexpr int ENC_POW2_ROW = 1024;
 
 // x >= c ? x - c : x
 EVAB_HD u64 csub(u64 x, u64 c) {

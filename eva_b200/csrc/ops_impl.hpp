@@ -16,7 +16,7 @@ struct CtxView {
   const u64 *zeros;         // [k]
   const cplx *roots;        // [N]   CKKS encoder tables
   const u32 *slot_index;    // [N]
-  const u64 *pow2;          // [k][128]
+  const u64 *pow2;          // [k][ENC_POW2_ROW]
   const u64x2 *qinv_f;      // [k][k]   fold rows of qinv
   unsigned foldmask;        // bit i: prime i is fold-friendly (modarith.cuh prime_foldable)
   const FoldPrime *fold_host;   // [k] HOST array: per-prime fold constants, copied into every NttLaunch

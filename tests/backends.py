@@ -32,14 +32,20 @@ def _elt(N, steps):
 
 class EmuBackend:
     name = "emu"
+    SRC, LIB = "emu.cpp", "libevab_emu"     # source under tests/emu and the library it builds
 
-    def __init__(self, N, primes, cluster=1):
-        so = os.path.join(ROOT, "tests", "emu", "libevab_emu.so")
-        src = os.path.join(ROOT, "tests", "emu", "emu.cpp")
-        deps = [src] + [os.path.join(ROOT, "eva_b200", "csrc", f) for f in os.listdir(os.path.join(ROOT, "eva_b200", "csrc"))]
+    def __init__(self, N, primes, cluster=1, bound_check=False):
+        """bound_check: a separately built library with -DEVAB_BOUND_CHECK, in which every compile-time bound of the fold
+        arithmetic is checked against the value it describes; a violated bound prints `bound violated at ...` and aborts the
+        process, so run it in a subprocess"""
+        so = os.path.join(ROOT, "tests", "emu", self.LIB + ("_bc.so" if bound_check else ".so"))
+        src = os.path.join(ROOT, "tests", "emu", self.SRC)
+        deps = [src, os.path.join(ROOT, "tests", "emu", "emu.cpp")] + [os.path.join(ROOT, "eva_b200", "csrc", f) for f in os.listdir(os.path.join(ROOT, "eva_b200", "csrc"))]
         if not os.path.exists(so) or any(os.path.getmtime(d) > os.path.getmtime(so) for d in deps):
-            subprocess.check_call(["g++", "-O2", "-std=c++17", "-fPIC", "-shared", "-ffp-contract=off", "-x", "c++", src, "-o", so])
+            defs = ["-DEVAB_BOUND_CHECK"] if bound_check else []
+            subprocess.check_call(["g++", "-O2", "-std=c++17", "-fPIC", "-shared", "-ffp-contract=off"] + defs + ["-x", "c++", src, "-o", so])
         self.lib = C.CDLL(so)
+        assert self.lib.emu_bound_checked() == int(bound_check)
         self.lib.emu_ctx_create.restype = C.c_void_p
         self.lib.emu_last_error.restype = C.c_char_p
         for n in ("emu_rescale_work_bytes", "emu_keyswitch_work_bytes", "emu_encode_work_bytes"):

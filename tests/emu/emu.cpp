@@ -230,6 +230,11 @@ void emu_ctx_destroy(EmuCtx *c) { delete c; }
 int emu_ctx_set_ntt_arith(EmuCtx *c, int mode) { c->v.arith = mode; return 0; }
 unsigned emu_ctx_foldmask(EmuCtx *c) { return c->v.foldmask; }
 int emu_fold_launches() { return g_folded; }
+#if defined(EVAB_BOUND_CHECK)
+int emu_bound_checked() { return 1; }   // this library verifies every tracked bound of the fold arithmetic (ntt_core.cuh)
+#else
+int emu_bound_checked() { return 0; }
+#endif
 int emu_ntt_fwd(EmuCtx *c, uint64_t *d, size_t count, const int *pidx, int np) { EmuBE be{c}; return ntt_batch_impl(be, c->v, false, d, count, pidx, np); }
 int emu_ntt_inv(EmuCtx *c, uint64_t *d, size_t count, const int *pidx, int np) { EmuBE be{c}; return ntt_batch_impl(be, c->v, true, d, count, pidx, np); }
 int emu_add(EmuCtx *c, int ell, uint64_t *o, const uint64_t *a, int sa, const uint64_t *b, int sb) { EmuBE be{c}; return dyadic_impl<DY_ADD>(be, c->v, ell, o, a, sa, b, sb, 0); }

@@ -1,14 +1,12 @@
 """Bit-exact weighted rotation sums (evab_rotate_wsum): the kernels on the CPU emulator and the GPU against the oracle, and the
 executor's rotation_sums plans (the default) against plans without them."""
 import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 import pytest
 
 import parity_cases as pc
-from backends import ROOT, EmuBackend, GpuBackend, _elt, _p
+from backends import EmuBackend, GpuBackend, _elt, _p
 from oracle import oracle as o
 
 
@@ -19,21 +17,12 @@ def _ptrs(xs):
 class WsumEmuBackend(EmuBackend):
     """EmuBackend plus evab_rotate_wsum replayed on the CPU (tests/emu/emu_wsum.cpp: emu.cpp + the new kernel body and the forward
     NTT with PRO_PLAIN + EPI_DIVROUND), in a library and context of its own"""
+    SRC, LIB = "emu_wsum.cpp", "libevab_emu_wsum"
 
-    def __init__(self, N, primes):
-        super().__init__(N, primes)
-        so = os.path.join(ROOT, "tests", "emu", "libevab_emu_wsum.so")
-        src = os.path.join(ROOT, "tests", "emu", "emu_wsum.cpp")
-        deps = [src, os.path.join(ROOT, "tests", "emu", "emu.cpp")] + [os.path.join(ROOT, "eva_b200", "csrc", f) for f in os.listdir(os.path.join(ROOT, "eva_b200", "csrc"))]
-        if not os.path.exists(so) or any(os.path.getmtime(d) > os.path.getmtime(so) for d in deps):
-            subprocess.check_call(["g++", "-O2", "-std=c++17", "-fPIC", "-shared", "-ffp-contract=off", "-x", "c++", src, "-o", so])
-        self.lib = C.CDLL(so)
-        self.lib.emu_ctx_create.restype = C.c_void_p
-        self.lib.emu_last_error.restype = C.c_char_p
+    def __init__(self, N, primes, bound_check=False):
+        super().__init__(N, primes, bound_check=bound_check)
         for fn in ("emu_rotate_modup_work_bytes", "emu_rotate_wsum_work_bytes"):
             getattr(self.lib, fn).restype = C.c_size_t
-        pa = np.array(primes, dtype=np.uint64)
-        self.h = C.c_void_p(self.lib.emu_ctx_create(C.c_uint64(N), _p(pa), len(primes)))
 
     def rotate_wsum(self, a, steps_list, gks, wts, taps, twts):
         """out_o = sum_i wts[o][i] (.) rotate(a, steps[i]) + sum_t twts[o][t] (.) taps[t] (scalar plaintexts [ell][N], None: weight 0).
