@@ -209,6 +209,11 @@ __global__ void __launch_bounds__(256, 4) k_rot_many(const RotManyArgs A, const 
   const int i = blockIdx.y / (A.ell + 1), mi = blockIdx.y % (A.ell + 1);
   for (int j = (blockIdx.x * blockDim.x + threadIdx.x) * 2; j < A.N; j += gridDim.x * blockDim.x * 2) rot_many_elem(A, i, mi, j, off);
 }
+// grid.y = row of the extended basis; every thread loops over the rotations, so blocks are kept small for more of them
+template <int NOUT> __global__ void __launch_bounds__(128) k_rot_wsum_ip(const WsumIpArgs A, const long long bstride) {
+  const long long off = (long long)blockIdx.z * bstride;
+  for (int j = (blockIdx.x * blockDim.x + threadIdx.x) * 2; j < A.N; j += gridDim.x * blockDim.x * 2) rot_wsum_ip_elem<NOUT>(A, blockIdx.y, j, off);
+}
 // grid.y = (polynomial, residue) of the outputs
 __global__ void __launch_bounds__(256) k_rot_wsum(const WsumArgs A, const long long bstride) {
   const long long off = (long long)blockIdx.z * bstride;
@@ -451,6 +456,19 @@ struct CudaBE {
   int rot_many(const RotManyArgs &A) {
     count();
     k_rot_many<<<grid(A.n * (A.ell + 1)), 256, 0, st>>>(A, g_batch.stride);
+    CUDA_OK(cudaGetLastError());
+    return 0;
+  }
+  int rot_wsum_ip(const WsumIpArgs &A) {
+    count();
+    const dim3 g(A.N / 2 / 128, A.ell + 1, g_batch.batch);   // N >= 1024
+    switch (A.nout) {
+      case 1: k_rot_wsum_ip<1><<<g, 128, 0, st>>>(A, g_batch.stride); break;
+      case 2: k_rot_wsum_ip<2><<<g, 128, 0, st>>>(A, g_batch.stride); break;
+      case 3: k_rot_wsum_ip<3><<<g, 128, 0, st>>>(A, g_batch.stride); break;
+      case 4: k_rot_wsum_ip<4><<<g, 128, 0, st>>>(A, g_batch.stride); break;
+      default: return fail("rotate_wsum: 1..4 output sums");
+    }
     CUDA_OK(cudaGetLastError());
     return 0;
   }

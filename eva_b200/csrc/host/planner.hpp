@@ -132,7 +132,7 @@ struct Plan {
   std::size_t cipherOps = 0;
   std::vector<const Term *> hoistSrc;           // hoist group -> the ciphertext its rotations read
   std::vector<std::size_t> hoistOff, hoistExtOff;   // arena word offsets of every hoist buffer and of its extended digits (hoistModUp)
-  std::vector<char> needsC0;                    // hoist group feeds evab_rotate_modup_many / a rotation sum
+  std::vector<char> needsC0;                    // hoist group feeds evab_rotate_modup_many / evab_lazy_rotsum
   std::vector<RotChunk> chunks;                 // rotationChunk
   std::unordered_map<std::uint64_t, int> chunkOf;
   std::vector<LazySum> lazy;                    // approxHoist / rotationSums
@@ -525,7 +525,8 @@ private:
     }
     p.needsC0.assign(p.hoistSrc.size(), 0);
     for (auto &ch : p.chunks) p.needsC0[ch.gid] = 1;
-    for (auto &L : p.lazy) p.needsC0[L.gid] = 1;
+    if (p.opt.approxHoist)   // evab_lazy_rotsum reads P * c0 on ext's diagonal; evab_rotate_wsum reads c0 itself
+      for (auto &L : p.lazy) p.needsC0[L.gid] = 1;
   }
 
   // ---- 6. Encode groups: one batched device encode per (ell, input-dependent?) group.

@@ -351,13 +351,31 @@ int rotate_modup_many_impl(BE &be, const CtxView &c, int ell, int n, u64 *out, c
 }
 
 // ---- rotate_wsum: out_o = sum_i w_oi (.) rotate(a, g_i) + sum_t w_ot (.) taps[t], every w a scalar plaintext [ell][N] (null: 0), in
-// four launches: the inner products of rotate_modup_many_impl, the inverse NTT of their 2n P rows, the weighting (k_rot_wsum, see
-// WsumArgs) and the forward NTT + division of the 2 nout ell weighted rows.  Same bits as rotate -> multiply_plain -> add: the
-// forward NTT is linear, so it commutes with the weighting, and every rotation keeps its own rounding by P.  n(2 + 2 ell)
-// transforms become 2n + 2 nout ell.  taps: size-2 ciphertexts at level ell (plain multiply_plain leaves of the sums).
-// out [nout][2][ell][N]; wts[o*n+i], twts[o*ntap+t]; work: rotate_wsum_work_elems.
+// four launches: the inner products of rotate_modup_many_impl with the weighting of their q rows (k_rot_wsum_ip: A, see WsumIpArgs),
+// the inverse NTT of their 2n P rows, the weighting of those (k_rot_wsum: D) and the forward NTT + division of the 2 nout ell
+// weighted rows.  Same bits as rotate -> multiply_plain -> add: the forward NTT is linear, so it commutes with the weighting, and
+// every rotation keeps its own rounding by P.  n(2 + 2 ell) transforms become 2n + 2 nout ell.  taps: size-2 ciphertexts at level
+// ell (plain multiply_plain leaves of the sums).  c0 is read from `a` itself: ext's diagonal (rotate_modup_scale_c0_impl) is not used.
+// out [nout][2][ell][N]; wts[o*n+i], twts[o*ntap+t]; work: rotate_wsum_work_elems = P rows [n][2] + tmp [n][2] + A, D [nout][2][ell].
 inline size_t rotate_wsum_work_elems(const CtxView &c, int ell, int n, int nout) {
-  return rotate_modup_many_work_elems(c, ell, n) + (size_t)2 * nout * 2 * ell * c.N;
+  return (size_t)2 * n * 2 * c.N + (size_t)2 * nout * 2 * ell * c.N;
+}
+// the inner products with the weighting: k_rot_wsum_ip in the CUDA build; compiled without CUDA (the CPU emulator of the tests) the
+// same element body replayed serially on the host
+template <class BE> int rot_wsum_ip_step(BE &be, const WsumIpArgs &A) {
+#if defined(__CUDACC__)
+  return be.rot_wsum_ip(A);
+#else
+  for (int mi = 0; mi <= A.ell; mi++)
+    for (int j = 0; j < A.N; j += 2) switch (A.nout) {
+        case 1: rot_wsum_ip_elem<1>(A, mi, j); break;
+        case 2: rot_wsum_ip_elem<2>(A, mi, j); break;
+        case 3: rot_wsum_ip_elem<3>(A, mi, j); break;
+        case 4: rot_wsum_ip_elem<4>(A, mi, j); break;
+        default: return be.error("rotate_wsum: 1..4 output sums");
+      }
+  return 0;
+#endif
 }
 template <class BE>
 int rotate_wsum_impl(BE &be, const CtxView &c, int ell, int nout, u64 *out, const u64 *a, const u64 *ext, int n, const u32 *const *perms,
@@ -368,23 +386,26 @@ int rotate_wsum_impl(BE &be, const CtxView &c, int ell, int nout, u64 *out, cons
   if (nout < 1 || nout > WS_OUT) return be.error("rotate_wsum: 1..4 output sums");
   if (ntap < 0 || ntap > WS_TAPS) return be.error("rotate_wsum: 0..16 plain taps");
   const long long N = (long long)c.N;
-  u64 *acc = work, *tmp = acc + (size_t)n * 2 * (ell + 1) * N;
+  u64 *prow = work, *tmp = prow + (size_t)n * 2 * N;
   u64 *A = tmp + (size_t)n * 2 * N, *D = A + (size_t)nout * 2 * ell * N;
-  RotManyArgs R;
+  WsumIpArgs R;
   memset(&R, 0, sizeof(R));
-  R.t = a + (size_t)ell * N; R.ext = ext; R.acc = acc; R.primes = c.primes; R.n = n; R.ell = ell; R.k = c.k; R.N = (int)N;
+  R.t = a + (size_t)ell * N; R.c0 = a; R.ext = ext; R.prow = prow; R.A = A; R.primes = c.primes;
+  R.n = n; R.ntap = ntap; R.nout = nout; R.ell = ell; R.k = c.k; R.N = (int)N;
   for (int i = 0; i < n; i++) { R.perm[i] = perms[i]; R.key[i] = keys[i]; R.cadd[i] = cadds[i]; }
-  if (int rc = be.rot_many(R)) return rc;
-  if (int rc = divround_inv_impl(be, c, acc, (long long)(ell + 1) * N, 2 * n, ell + 1, c.k - 1, tmp)) return rc;
+  for (int o = 0; o < nout; o++) {
+    for (int i = 0; i < n; i++) R.wt[o][i] = wts[(size_t)o * n + i];
+    for (int t = 0; t < ntap; t++) R.twt[o][t] = twts[(size_t)o * ntap + t];
+  }
+  for (int t = 0; t < ntap; t++) R.tap[t] = taps[t];
+  if (int rc = rot_wsum_ip_step(be, R)) return rc;
+  if (int rc = divround_inv_impl(be, c, prow, N, 2 * n, 1, c.k - 1, tmp)) return rc;
   WsumArgs W;
   memset(&W, 0, sizeof(W));
-  W.acc = acc; W.tmp = tmp; W.A = A; W.D = D; W.primes = c.primes; W.halfmod = c.halfmod + (size_t)(c.k - 1) * c.k;
-  W.n = n; W.ntap = ntap; W.nout = nout; W.ell = ell; W.k = c.k; W.N = (int)N;
-  for (int o = 0; o < nout; o++) {
+  W.tmp = tmp; W.D = D; W.primes = c.primes; W.halfmod = c.halfmod + (size_t)(c.k - 1) * c.k;
+  W.n = n; W.nout = nout; W.ell = ell; W.k = c.k; W.N = (int)N;
+  for (int o = 0; o < nout; o++)
     for (int i = 0; i < n; i++) W.wt[o][i] = wts[(size_t)o * n + i];
-    for (int t = 0; t < ntap; t++) W.twt[o][t] = twts[(size_t)o * ntap + t];
-  }
-  for (int t = 0; t < ntap; t++) W.tap[t] = taps[t];
   if (int rc = be.rot_wsum(W)) return rc;
   NttLaunch B = base_launch(c);
   B.src = D; B.src_sq = ell * N; B.src_sr = N;

@@ -287,64 +287,126 @@ EVAB_HD void hoist_indicator_elem(u64 *out, const u32 *ctab, int N, int mi, int 
 //   A[o][c][r] = sum_i w_oir acc_i[c][r] + sum_t (P mod q_r) w_otr x_t[c][r]     (folded plain taps: divided by P they give w x_t)
 //   D[o][c][r] = sum_i w_oir ((tmp_i[c] mod q_r) - floor(P/2) mod q_r)
 // and the forward NTT of D with the division epilogue (A - NTT(D)) P^-1 gives sum_i w_oi rotate(x, g_i) + sum_t w_ot x_t, the
-// rounding of every rotation being its own.  Products are accumulated in 128 bits and reduced once per output word: tmp_i < P
+// rounding of every rotation being its own.  A is formed inside the key-switch inner product (rot_wsum_ip_elem): the q rows of
+// acc_i are weighted where they are computed and never stored; only the P rows are, for the inverse NTT that tmp_i comes from.
+// D follows that transform (rot_wsum_elem).  Products are accumulated in 128 bits and reduced once per output word: tmp_i < P
 // enters unreduced, and -floor(P/2) as + (q_r - floor(P/2) mod q_r), the same residue as pro_load's MODRED; every product is
 // below 2^121 (primes < 2^60), so the WS_MAX + WS_TAPS products of one output word fit.
 #define WS_MAX 16
 #define WS_TAPS 16
 #define WS_OUT 4
-struct WsumArgs {
-  const u64 *acc;                  // [n][2][ell+1][N] (k_rot_many)
-  const u64 *tmp;                  // [n][2][N]        (inverse NTT of the P rows, + floor(P/2))
+struct WsumIpArgs {
+  const u64 *t, *c0, *ext;         // source c1 / c0 [ell][N], shared extended digits [ell+1][ell][N] (the diagonal is not read)
+  const u32 *perm[WS_MAX];
+  const u64 *key[WS_MAX], *cadd[WS_MAX];
   const u64 *wt[WS_OUT][WS_MAX];   // scalar plaintexts [ell][N] (batch instance offset applies); null: weight 0
   const u64 *tap[WS_TAPS];         // size-2 ciphertexts [2][ell][N] at the output's level (batch instance offset applies)
   const u64 *twt[WS_OUT][WS_TAPS]; // their scalar weights; null: weight 0
-  u64 *A, *D;                      // [nout][2][ell][N]
+  u64 *prow;                       // [n][2][N]        the P rows of the accumulators
+  u64 *A;                          // [nout][2][ell][N]
   const PrimeDev *primes;
-  const u64 *halfmod;              // [k]: floor(P/2) mod q_r
   int n, ntap, nout, ell, k, N;
 };
-// coefficients j, j+1 of residue r of polynomial c of every output
+// coefficients j, j+1 of row mi (q_0 .. q_{ell-1}, P) of both polynomials, every rotation and every output (nout == NOUT).  acc_i is
+// rot_many_elem's canonical value: the inner product through perm_i + cadd_i, and on a q row + perm_i(P c0) = (P mod q_m) c0[perm_i(j)],
+// read from c0 directly.  A P row is stored; a q row is weighted into A, which then takes the taps.
+template <int NOUT> EVAB_HD void rot_wsum_ip_elem(const WsumIpArgs &A, int mi, int j, long long off = 0) {
+  const bool qrow = mi < A.ell;
+  const int row = qrow ? mi : A.k - 1;
+  const PrimeDev P = A.primes[row];
+  const size_t N = A.N;
+  const u64 pm = qrow ? barrett64(A.primes[A.k - 1].p, P.p, P.ratio64) : 0;   // P mod q_m
+  const u64 *c0p = A.c0 + off + (size_t)mi * N;
+  u64 al[NOUT][2][2], ah[NOUT][2][2];   // [output][polynomial][coefficient]
+#pragma unroll
+  for (int o = 0; o < NOUT; o++)
+#pragma unroll
+    for (int c = 0; c < 2; c++) al[o][c][0] = al[o][c][1] = ah[o][c][0] = ah[o][c][1] = 0;
+  u32 pj0 = EVAB_LDG(A.perm[0] + j), pj1 = EVAB_LDG(A.perm[0] + j + 1);
+  for (int i = 0; i < A.n; i++) {
+    const u32 p0 = pj0, p1 = pj1;
+    if (i + 1 < A.n) { pj0 = EVAB_LDG(A.perm[i + 1] + j); pj1 = EVAB_LDG(A.perm[i + 1] + j + 1); }   // the next gather's addresses
+    u64 l0x = 0, h0x = 0, l0y = 0, h0y = 0, l1x = 0, h1x = 0, l1y = 0, h1y = 0;
+    for (int J = 0; J < A.ell; J++) {
+      const u64 *src = (row == J) ? A.t + off + (size_t)J * N : A.ext + off + ((size_t)mi * A.ell + J) * N;
+      const u64 vx = EVAB_LDG(src + p0), vy = EVAB_LDG(src + p1);
+      const u64x2 k0 = ld2(A.key[i] + (((size_t)J * 2 + 0) * A.k + row) * N + j);
+      const u64x2 k1 = ld2(A.key[i] + (((size_t)J * 2 + 1) * A.k + row) * N + j);
+      mac128(l0x, h0x, vx, k0.x); mac128(l0y, h0y, vy, k0.y);
+      mac128(l1x, h1x, vx, k1.x); mac128(l1y, h1y, vy, k1.y);
+    }
+    const u64x2 c0 = ld2(A.cadd[i] + ((size_t)0 * (A.ell + 1) + mi) * N + j), c1 = ld2(A.cadd[i] + ((size_t)1 * (A.ell + 1) + mi) * N + j);
+    u64x2 r0, r1;
+    r0.x = addmod(reduce128(l0x, h0x, P), c0.x, P.p); r0.y = addmod(reduce128(l0y, h0y, P), c0.y, P.p);
+    r1.x = addmod(reduce128(l1x, h1x, P), c1.x, P.p); r1.y = addmod(reduce128(l1y, h1y, P), c1.y, P.p);
+    if (!qrow) {
+      st2(A.prow + off + ((size_t)i * 2 + 0) * N + j, r0);
+      st2(A.prow + off + ((size_t)i * 2 + 1) * N + j, r1);
+      continue;
+    }
+    r0.x = addmod(r0.x, mulmod_p(EVAB_LDG(c0p + p0), pm, P), P.p);
+    r0.y = addmod(r0.y, mulmod_p(EVAB_LDG(c0p + p1), pm, P), P.p);
+#pragma unroll
+    for (int o = 0; o < NOUT; o++) {
+      if (!A.wt[o][i]) continue;
+      const u64 w = EVAB_LDG(A.wt[o][i] + off + (size_t)mi * N);
+      mac128(al[o][0][0], ah[o][0][0], r0.x, w); mac128(al[o][0][1], ah[o][0][1], r0.y, w);
+      mac128(al[o][1][0], ah[o][1][0], r1.x, w); mac128(al[o][1][1], ah[o][1][1], r1.y, w);
+    }
+  }
+  if (!qrow) return;
+  for (int t = 0; t < A.ntap; t++) {
+    const u64x2 x0 = ld2(A.tap[t] + off + (size_t)mi * N + j), x1 = ld2(A.tap[t] + off + ((size_t)A.ell + mi) * N + j);
+#pragma unroll
+    for (int o = 0; o < NOUT; o++) {
+      if (!A.twt[o][t]) continue;
+      const u64 w = mulmod_p(pm, EVAB_LDG(A.twt[o][t] + off + (size_t)mi * N), P);
+      mac128(al[o][0][0], ah[o][0][0], x0.x, w); mac128(al[o][0][1], ah[o][0][1], x0.y, w);
+      mac128(al[o][1][0], ah[o][1][0], x1.x, w); mac128(al[o][1][1], ah[o][1][1], x1.y, w);
+    }
+  }
+#pragma unroll
+  for (int o = 0; o < NOUT; o++)
+#pragma unroll
+    for (int c = 0; c < 2; c++) {
+      u64x2 v;
+      v.x = reduce128(al[o][c][0], ah[o][c][0], P); v.y = reduce128(al[o][c][1], ah[o][c][1], P);
+      st2(A.A + off + (((size_t)o * 2 + c) * A.ell + mi) * N + j, v);
+    }
+}
+
+struct WsumArgs {
+  const u64 *tmp;                  // [n][2][N]        (inverse NTT of the P rows, + floor(P/2))
+  const u64 *wt[WS_OUT][WS_MAX];   // scalar plaintexts [ell][N] (batch instance offset applies); null: weight 0
+  u64 *D;                          // [nout][2][ell][N]
+  const PrimeDev *primes;
+  const u64 *halfmod;              // [k]: floor(P/2) mod q_r
+  int n, nout, ell, k, N;
+};
+// D: coefficients j, j+1 of residue r of polynomial c of every output
 EVAB_HD void rot_wsum_elem(const WsumArgs &A, int c, int r, int j, long long off = 0) {
   const PrimeDev P = A.primes[r];
   const size_t N = A.N;
   const u64 nh = P.p - A.halfmod[r];
-  u64 al[WS_OUT][2], ah[WS_OUT][2], dl[WS_OUT][2], dh[WS_OUT][2];
+  u64 dl[WS_OUT][2], dh[WS_OUT][2];
 #pragma unroll
-  for (int o = 0; o < WS_OUT; o++) al[o][0] = al[o][1] = ah[o][0] = ah[o][1] = dl[o][0] = dl[o][1] = dh[o][0] = dh[o][1] = 0;
+  for (int o = 0; o < WS_OUT; o++) dl[o][0] = dl[o][1] = dh[o][0] = dh[o][1] = 0;
   for (int i = 0; i < A.n; i++) {
-    const u64x2 a = ld2(A.acc + off + (((size_t)i * 2 + c) * (A.ell + 1) + r) * N + j);
     u64x2 t = ld2(A.tmp + off + ((size_t)i * 2 + c) * N + j);
     t.x += nh; t.y += nh;
 #pragma unroll
     for (int o = 0; o < WS_OUT; o++) {
       if (o >= A.nout || !A.wt[o][i]) continue;
       const u64 w = EVAB_LDG(A.wt[o][i] + off + (size_t)r * N);
-      mac128(al[o][0], ah[o][0], a.x, w); mac128(al[o][1], ah[o][1], a.y, w);
       mac128(dl[o][0], dh[o][0], t.x, w); mac128(dl[o][1], dh[o][1], t.y, w);
-    }
-  }
-  if (A.ntap) {
-    const u64 pm = barrett64(A.primes[A.k - 1].p, P.p, P.ratio64);   // P mod q_r
-    for (int t = 0; t < A.ntap; t++) {
-      const u64x2 x = ld2(A.tap[t] + off + ((size_t)c * A.ell + r) * N + j);
-#pragma unroll
-      for (int o = 0; o < WS_OUT; o++) {
-        if (o >= A.nout || !A.twt[o][t]) continue;
-        const u64 w = mulmod_p(pm, EVAB_LDG(A.twt[o][t] + off + (size_t)r * N), P);
-        mac128(al[o][0], ah[o][0], x.x, w); mac128(al[o][1], ah[o][1], x.y, w);
-      }
     }
   }
 #pragma unroll
   for (int o = 0; o < WS_OUT; o++) {
     if (o >= A.nout) break;
-    const size_t w = off + (((size_t)o * 2 + c) * A.ell + r) * N + j;
     u64x2 v;
-    v.x = reduce128(al[o][0], ah[o][0], P); v.y = reduce128(al[o][1], ah[o][1], P);
-    st2(A.A + w, v);
     v.x = reduce128(dl[o][0], dh[o][0], P); v.y = reduce128(dl[o][1], dh[o][1], P);
-    st2(A.D + w, v);
+    st2(A.D + off + (((size_t)o * 2 + c) * A.ell + r) * N + j, v);
   }
 }
 

@@ -197,8 +197,8 @@ int evab_rotate_modup_prepared(evab_ctx *ctx, int ell, uint64_t *d_out, const ui
                                const uint64_t *d_key, const uint64_t *d_cadd, void *d_work, void *stream);
 /* n <= 16 rotations of ONE ciphertext (seal::Evaluator::rotate_vector, seal_executor.h:176-189) in three kernel launches instead of
  * 3 n: d_out [n][2][ell][N], rotation i by galois_elts[i]; same bits as n calls of evab_rotate_modup_prepared.  d_ext, keys, cadds as there. */
-/* evab_rotate_modup_many, evab_rotate_wsum and evab_lazy_rotsum read P * c0 from the diagonal of d_ext (ext[m][J] has no entry for m = q_J): call this once
- * per ciphertext after evab_rotate_modup_prepare and before either of them. */
+/* evab_rotate_modup_many and evab_lazy_rotsum read P * c0 from the diagonal of d_ext (ext[m][J] has no entry for m = q_J): call this once
+ * per ciphertext after evab_rotate_modup_prepare and before either of them.  evab_rotate_wsum does not need it (it reads c0 itself). */
 int evab_rotate_modup_scale_c0(evab_ctx *ctx, int ell, uint64_t *d_ext, const uint64_t *d_a, void *stream);
 size_t evab_rotate_modup_many_work_bytes(const evab_ctx *ctx, int ell, int n);
 int evab_rotate_modup_many(evab_ctx *ctx, int ell, int n, uint64_t *d_out, const uint64_t *d_a, const uint64_t *d_ext, const uint64_t *galois_elts,
@@ -208,7 +208,7 @@ int evab_rotate_modup_many(evab_ctx *ctx, int ell, int n, uint64_t *d_out, const
  * rotate -> multiply_plain -> add (every rotation keeps its own rounding by P), in four launches and 2 n + 2 nout ell transforms instead of
  * n (2 + 2 ell).  Every weight is a SCALAR plaintext [ell][N] (the encoding of a replicated constant: one value per residue);
  * d_wts[o * n + i] weighs rotation i in sum o, d_twts[o * ntap + t] tap t, NULL for weight 0.  d_ext, keys, cadds as for
- * evab_rotate_modup_many (after evab_rotate_modup_scale_c0). */
+ * evab_rotate_modup_many; the diagonal of d_ext is not read. */
 size_t evab_rotate_wsum_work_bytes(const evab_ctx *ctx, int ell, int n, int nout);
 int evab_rotate_wsum(evab_ctx *ctx, int ell, int nout, uint64_t *d_out, const uint64_t *d_a, const uint64_t *d_ext, int n, const uint64_t *galois_elts,
                      const uint64_t *const *d_keys, const uint64_t *const *d_cadds, const uint64_t *const *d_wts, int ntap,
