@@ -80,6 +80,7 @@ _SIGS = {
     "evab_rescale": (ci, [vp, ci, vp, vp, ci, vp, vp]),
     "evab_copy": (ci, [vp, ci, vp, vp, ci, vp]),
     "evab_set_batch": (ci, [ci, szt, szt]),
+    "evab_set_key_bank": (ci, [vp, szt]),
     "evab_mod_switch": (ci, [vp, ci, vp, vp, ci, vp]),
     "evab_keyswitch_work_bytes": (szt, [vp, ci]),
     "evab_relinearize": (ci, [vp, ci, vp, vp, vp, vp, vp]),

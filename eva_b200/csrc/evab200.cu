@@ -55,6 +55,14 @@ extern "C" int evab_set_batch(int batch, size_t stride_words, size_t value_strid
   g_batch.batch = batch; g_batch.stride = (long long)stride_words; g_batch.vstride = (long long)value_stride;
   return 0;
 }
+// thread-local key selection (evab_set_key_bank): instance b reads its keys at + tenant[b] * stride words
+struct KeyBankSel { const int32_t *tenant = nullptr; long long stride = 0; };
+static thread_local KeyBankSel g_bank;
+extern "C" int evab_set_key_bank(const int32_t *d_tenant_of_instance, size_t tenant_stride_words) {
+  g_bank.tenant = d_tenant_of_instance;
+  g_bank.stride = d_tenant_of_instance ? (long long)tenant_stride_words : 0;
+  return 0;
+}
 
 
 // ---------------------------------------------------------------------------
@@ -195,24 +203,27 @@ __global__ void __launch_bounds__(256) k_sum_terms(const SumArgs A, const long l
   for (int j = (blockIdx.x * blockDim.x + threadIdx.x) * 2; j < A.N; j += gridDim.x * blockDim.x * 2)
     sum_terms_elem(A, blockIdx.y, j, off);
 }
-__global__ void __launch_bounds__(256) k_ks_inner(const IpArgs A, const long long bstride) {
+// key offset of this block's instance: BANK = false is the shared-key launch (offset 0, the table is not read)
+template <bool BANK> __device__ __forceinline__ long long key_off(const KeyBankSel &K) { return BANK ? (long long)__ldg(K.tenant + blockIdx.z) * K.stride : 0; }
+template <bool BANK> __global__ void __launch_bounds__(256) k_ks_inner(const IpArgs A, const long long bstride, const KeyBankSel K) {
   const long long off = (long long)blockIdx.z * bstride;   // parameters stay in constant memory: no local copy
+  const long long koff = key_off<BANK>(K);
   for (int j = (blockIdx.x * blockDim.x + threadIdx.x) * 2; j < A.N; j += gridDim.x * blockDim.x * 2)
-    ks_inner_elem(A, blockIdx.y, j, off);
+    ks_inner_elem(A, blockIdx.y, j, off, koff);
 }
 __global__ void __launch_bounds__(256) k_scale_c0(const u64 *c0, u64 *ext, const PrimeDev *primes, int ell, int k, int N, const long long bstride) {
   const long long off = (long long)blockIdx.z * bstride;
   for (int j = blockIdx.x * blockDim.x + threadIdx.x; j < N; j += gridDim.x * blockDim.x) scale_c0_elem(c0, ext, primes, ell, k, N, blockIdx.y, j, off);
 }
-__global__ void __launch_bounds__(256, 4) k_rot_many(const RotManyArgs A, const long long bstride) {
-  const long long off = (long long)blockIdx.z * bstride;
+template <bool BANK> __global__ void __launch_bounds__(256, 4) k_rot_many(const RotManyArgs A, const long long bstride, const KeyBankSel K) {
+  const long long off = (long long)blockIdx.z * bstride, koff = key_off<BANK>(K);
   const int i = blockIdx.y / (A.ell + 1), mi = blockIdx.y % (A.ell + 1);
-  for (int j = (blockIdx.x * blockDim.x + threadIdx.x) * 2; j < A.N; j += gridDim.x * blockDim.x * 2) rot_many_elem(A, i, mi, j, off);
+  for (int j = (blockIdx.x * blockDim.x + threadIdx.x) * 2; j < A.N; j += gridDim.x * blockDim.x * 2) rot_many_elem(A, i, mi, j, off, koff);
 }
 // grid.y = row of the extended basis; every thread loops over the rotations, so blocks are kept small for more of them
-template <int NOUT> __global__ void __launch_bounds__(128) k_rot_wsum_ip(const WsumIpArgs A, const long long bstride) {
-  const long long off = (long long)blockIdx.z * bstride;
-  for (int j = (blockIdx.x * blockDim.x + threadIdx.x) * 2; j < A.N; j += gridDim.x * blockDim.x * 2) rot_wsum_ip_elem<NOUT>(A, blockIdx.y, j, off);
+template <int NOUT, bool BANK> __global__ void __launch_bounds__(128) k_rot_wsum_ip(const WsumIpArgs A, const long long bstride, const KeyBankSel K) {
+  const long long off = (long long)blockIdx.z * bstride, koff = key_off<BANK>(K);
+  for (int j = (blockIdx.x * blockDim.x + threadIdx.x) * 2; j < A.N; j += gridDim.x * blockDim.x * 2) rot_wsum_ip_elem<NOUT>(A, blockIdx.y, j, off, koff);
 }
 // grid.y = (polynomial, residue) of the outputs
 __global__ void __launch_bounds__(256) k_rot_wsum(const WsumArgs A, const long long bstride) {
@@ -221,12 +232,12 @@ __global__ void __launch_bounds__(256) k_rot_wsum(const WsumArgs A, const long l
   for (int j = (blockIdx.x * blockDim.x + threadIdx.x) * 2; j < A.N; j += gridDim.x * blockDim.x * 2) rot_wsum_elem(A, c, r, j, off);
 }
 // block = 32 element pairs x n rotations (one warp per rotation); the parts meet in shared memory, one output sum at a time
-__global__ void __launch_bounds__(32 * LRS_MAX) k_lazy_rotsum(const LazyRotSumArgs A, const long long bstride) {
+template <bool BANK> __global__ void __launch_bounds__(32 * LRS_MAX) k_lazy_rotsum(const LazyRotSumArgs A, const long long bstride, const KeyBankSel K) {
   __shared__ u64 sh[LRS_MAX][4][32];
   const long long off = (long long)blockIdx.z * bstride;
   const int j = (blockIdx.x * 32 + threadIdx.x) * 2, i = threadIdx.y, mi = blockIdx.y;
   u64 part[LRS_OUT][4];
-  lazy_rotsum_part(A, mi, j, i, off, part);
+  lazy_rotsum_part(A, mi, j, i, off, part, key_off<BANK>(K));
 #pragma unroll
   for (int o = 0; o < LRS_OUT; o++) {
     if (o >= A.nout) break;
@@ -443,7 +454,8 @@ struct CudaBE {
   }
   int inner(const IpArgs &A) {
     count();
-    k_ks_inner<<<grid(A.ell + 1), 256, 0, st>>>(A, g_batch.stride);
+    if (g_bank.tenant) k_ks_inner<true><<<grid(A.ell + 1), 256, 0, st>>>(A, g_batch.stride, g_bank);
+    else k_ks_inner<false><<<grid(A.ell + 1), 256, 0, st>>>(A, g_batch.stride, g_bank);
     CUDA_OK(cudaGetLastError());
     return 0;
   }
@@ -455,18 +467,24 @@ struct CudaBE {
   }
   int rot_many(const RotManyArgs &A) {
     count();
-    k_rot_many<<<grid(A.n * (A.ell + 1)), 256, 0, st>>>(A, g_batch.stride);
+    if (g_bank.tenant) k_rot_many<true><<<grid(A.n * (A.ell + 1)), 256, 0, st>>>(A, g_batch.stride, g_bank);
+    else k_rot_many<false><<<grid(A.n * (A.ell + 1)), 256, 0, st>>>(A, g_batch.stride, g_bank);
     CUDA_OK(cudaGetLastError());
     return 0;
   }
   int rot_wsum_ip(const WsumIpArgs &A) {
     count();
     const dim3 g(A.N / 2 / 128, A.ell + 1, g_batch.batch);   // N >= 1024
-    switch (A.nout) {
-      case 1: k_rot_wsum_ip<1><<<g, 128, 0, st>>>(A, g_batch.stride); break;
-      case 2: k_rot_wsum_ip<2><<<g, 128, 0, st>>>(A, g_batch.stride); break;
-      case 3: k_rot_wsum_ip<3><<<g, 128, 0, st>>>(A, g_batch.stride); break;
-      case 4: k_rot_wsum_ip<4><<<g, 128, 0, st>>>(A, g_batch.stride); break;
+    const bool bank = g_bank.tenant != nullptr;
+    switch (A.nout * 2 + bank) {
+      case 2: k_rot_wsum_ip<1, false><<<g, 128, 0, st>>>(A, g_batch.stride, g_bank); break;
+      case 3: k_rot_wsum_ip<1, true><<<g, 128, 0, st>>>(A, g_batch.stride, g_bank); break;
+      case 4: k_rot_wsum_ip<2, false><<<g, 128, 0, st>>>(A, g_batch.stride, g_bank); break;
+      case 5: k_rot_wsum_ip<2, true><<<g, 128, 0, st>>>(A, g_batch.stride, g_bank); break;
+      case 6: k_rot_wsum_ip<3, false><<<g, 128, 0, st>>>(A, g_batch.stride, g_bank); break;
+      case 7: k_rot_wsum_ip<3, true><<<g, 128, 0, st>>>(A, g_batch.stride, g_bank); break;
+      case 8: k_rot_wsum_ip<4, false><<<g, 128, 0, st>>>(A, g_batch.stride, g_bank); break;
+      case 9: k_rot_wsum_ip<4, true><<<g, 128, 0, st>>>(A, g_batch.stride, g_bank); break;
       default: return fail("rotate_wsum: 1..4 output sums");
     }
     CUDA_OK(cudaGetLastError());
@@ -480,7 +498,9 @@ struct CudaBE {
   }
   int lazy_rotsum(const LazyRotSumArgs &A) {
     count();
-    k_lazy_rotsum<<<dim3(A.N / 64, A.ell + 1, g_batch.batch), dim3(32, A.n), 0, st>>>(A, g_batch.stride);
+    const dim3 g(A.N / 64, A.ell + 1, g_batch.batch), b(32, A.n);
+    if (g_bank.tenant) k_lazy_rotsum<true><<<g, b, 0, st>>>(A, g_batch.stride, g_bank);
+    else k_lazy_rotsum<false><<<g, b, 0, st>>>(A, g_batch.stride, g_bank);
     CUDA_OK(cudaGetLastError());
     return 0;
   }

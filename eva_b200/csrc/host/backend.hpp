@@ -53,7 +53,8 @@ struct Shared {
   std::shared_ptr<Device> dev;
   std::unique_ptr<CkksClient> client;
   KeySet keys;
-  std::mutex execMutex;   // serialises execute / executeMany callers of one context (see executeMany)
+  std::unique_ptr<KeyBank> bank;   // B200Server: the tenants' keys (then `keys` is empty and every batch names a tenant per instance)
+  std::mutex execMutex;   // serialises execute / executeMany callers of one context (see executeMany), and key-bank changes
 };
 
 // the cached plan of one (program, context) pair; owned by the Program
@@ -71,6 +72,7 @@ struct PendingBatch {
   std::vector<B200Valuation> outs;
   std::vector<void *> streams;
   std::vector<std::shared_ptr<PlanHolder>> plans;   // the plans it runs on stay alive until it is collected (set_options may replace them meanwhile)
+  std::vector<int> tenants;                         // key-bank tenant of every instance (B200Server), empty with a single key set
   int slot = 0;
   bool collected = false;
   std::shared_ptr<Shared> keep;
@@ -136,8 +138,9 @@ public:
       ExecOptions o = options;
       o.batch = batch;
       h->opt = o;   // as requested (what the staleness test above compares)
-      h->exec = std::make_unique<Executor>(s_->dev, s_->keys, program, o);
+      h->exec = std::make_unique<Executor>(s_->dev, s_->keys, program, o, s_->bank.get());
       h->termCount = program.termCount();
+      plansBuilt++;
       program.attach(key, h);
     }
     return h;
@@ -199,16 +202,19 @@ public:
   // Pipelined form of executeMany: submitMany enqueues a batch (H2D of its inputs, the plan replays, D2H of its outputs) and returns;
   // collect waits for it and hands out the results.  Batches submitted with different `slot` numbers (0..7) use disjoint plan
   // replicas, so the head of one overlaps the tail of the other (each batch alone ramps up replica by replica and drains the same way).
-  std::shared_ptr<PendingBatch> submitMany(Program &program, const std::vector<const B200Valuation *> &inputs, int slot = 0) {
+  // tenants: with a key bank (B200Server), the tenant whose keys instance b runs with; otherwise empty
+  std::shared_ptr<PendingBatch> submitMany(Program &program, const std::vector<const B200Valuation *> &inputs, int slot = 0, std::vector<int> tenants = {}) {
     if (inputs.empty()) throw std::invalid_argument("execute needs at least one valuation");
     if (slot < 0 || slot > 7) throw std::invalid_argument("slot out of range (0..7)");
+    if (s_->bank ? tenants.size() != inputs.size() : !tenants.empty()) throw std::invalid_argument("one tenant per valuation on a key bank, none otherwise");
     for (auto *v : inputs) requireAllInputs(program, *v);
     // one caller at a time per context: plan replicas own single arenas and raw-input buffers (the reference's
     // execute is re-entrant because it builds a new executor per call; concurrent callers are serialised here)
     std::lock_guard<std::mutex> guard(s_->execMutex);
+    for (int t : tenants) s_->bank->requireOccupied(t);
     if (auto prev = inFlight_[slot].lock(); prev && !prev->collected) throw std::runtime_error("slot in use: collect the batch submitted before");
     auto p = std::make_shared<PendingBatch>();
-    p->program = &program; p->inputs = inputs; p->slot = slot; p->keep = s_;
+    p->program = &program; p->inputs = inputs; p->slot = slot; p->keep = s_; p->tenants = std::move(tenants);
     enqueueLocked(*p);
     inFlight_[slot] = p;
     return p;
@@ -272,6 +278,7 @@ public:
       void *st = ex.mainStream();
       if (busy[r]) s_->dev->sync(st);   // the replica's arena is reused: wait for its previous chunk
       busy[r] = 1;
+      if (!p.tenants.empty()) ex.setTenants(p.tenants.data() + b0, nb);
       if (std::find(streams.begin(), streams.end(), st) == streams.end()) streams.push_back(st);
       if (std::find(p.plans.begin(), p.plans.end(), holder) == p.plans.end()) p.plans.push_back(holder);
       auto t1 = now();
@@ -302,13 +309,70 @@ public:
       std::fprintf(stderr, "[evab] enqueue B=%d F=%d slot=%d: plan %.3f stage %.3f run %.3f enqueue-total %.3f ms\n", B, F, p.slot, tPlan * 1e3, tStage * 1e3, tRun * 1e3,
                    std::chrono::duration<double>(now() - t00).count() * 1e3);
   }
+  // with execMutex held: does a submitted, not yet collected batch run an instance with this tenant's keys?
+  bool tenantInFlightLocked(int t) const {
+    for (auto &w : inFlight_)
+      if (auto p = w.lock(); p && !p->collected && std::find(p->tenants.begin(), p->tenants.end(), t) != p->tenants.end()) return true;
+    return false;
+  }
   std::shared_ptr<Shared> shared() const { return s_; }
   ExecOptions options;
+  std::uint64_t plansBuilt = 0;   // executors constructed by this context (plan build + arena + graph capture each)
 
 private:
   std::shared_ptr<Shared> s_;
   std::uint64_t id_ = 0;
   std::weak_ptr<PendingBatch> inFlight_[8];
+};
+
+// One device and one parameter set serving many clients: each client's evaluation keys are a tenant of a key bank, the plans of
+// a program belong to the server (built, allocated and captured once, whatever the number of tenants), and every instance of a
+// batch runs with its own tenant's keys.  Execution is B200Public's (replicas, slots, fused chunks, the zero-digit redo).
+class B200Server {
+public:
+  B200Server(const CKKSParameters &params, int capacity, int device) {
+    std::vector<int> bits(params.primeBits.begin(), params.primeBits.end());
+    auto s = std::make_shared<Shared>();
+    s->dev = std::make_shared<Device>(params.polyModulusDegree, hmod::createCoeffModulus(params.polyModulusDegree, bits), device);
+    s->client = std::make_unique<CkksClient>(s->dev, 0);
+    std::set<u64> elts;
+    for (int step : params.rotations) {
+      const u64 elt = evab_galois_elt_from_step(params.polyModulusDegree, step);
+      if (!elt) throw std::invalid_argument("step count too large");
+      elts.insert(elt);
+    }
+    s->bank = std::make_unique<KeyBank>(s->dev, elts, capacity);
+    pub_ = std::make_unique<B200Public>(s);
+  }
+  // host images [k-1][2][k][N] (shapes checked by the caller); every element of the rotation set must be present
+  int addKeys(const u64 *relin, const std::map<u64, const u64 *> &galois) {
+    for (u64 e : bank().elements())
+      if (!galois.count(e)) throw std::invalid_argument("Galois key for element " + std::to_string(e) + " of the server's rotation set is missing");
+    std::lock_guard<std::mutex> guard(shared()->execMutex);
+    return shared()->bank->add(relin, galois);
+  }
+  void removeKeys(int t) {
+    std::lock_guard<std::mutex> guard(shared()->execMutex);
+    shared()->bank->requireOccupied(t);
+    if (pub_->tenantInFlightLocked(t)) throw std::runtime_error("tenant " + std::to_string(t) + " is used by a batch that has not been collected");
+    shared()->bank->remove(t);
+  }
+  std::shared_ptr<PendingBatch> submit(Program &program, const std::vector<std::pair<int, const B200Valuation *>> &requests, int slot = 0) {
+    std::vector<const B200Valuation *> in;
+    std::vector<int> tenants;
+    for (auto &r : requests) { tenants.push_back(r.first); in.push_back(r.second); }
+    return pub_->submitMany(program, in, slot, std::move(tenants));
+  }
+  std::vector<B200Valuation> executeBatch(Program &program, const std::vector<std::pair<int, const B200Valuation *>> &requests) {
+    auto p = submit(program, requests, 0);
+    return pub_->collect(*p);
+  }
+  B200Public &pub() { return *pub_; }
+  const KeyBank &bank() const { return *pub_->shared()->bank; }
+  std::shared_ptr<Shared> shared() const { return pub_->shared(); }
+
+private:
+  std::unique_ptr<B200Public> pub_;
 };
 
 class B200Secret {

@@ -24,16 +24,95 @@ struct BatchGuard {
   BatchGuard(int batch, std::size_t stride, std::size_t vstride) { check(evab_set_batch(batch, stride, vstride)); }
   ~BatchGuard() { evab_set_batch(1, 0, 0); }
 };
+// scoped evab_set_key_bank: batch instance b of the ops issued by this thread reads the keys of tenant d_tenant[b] (null: shared keys)
+struct KeyBankGuard {
+  KeyBankGuard(const std::int32_t *d_tenant, std::size_t stride) { check(evab_set_key_bank(d_tenant, stride)); }
+  ~KeyBankGuard() { evab_set_key_bank(nullptr, 0); }
+};
+
+// Evaluation keys of up to `capacity` tenants (one client's key set each) in one device allocation.  Every tenant's region has
+// the same layout -- the relinearization key, one Galois key per element of the rotation set, then the hoist constants cadd of
+// every (element, ell) with ell = 1 .. k-1 (evab_rotate_hoist_const, filled when the tenant is added) -- so tenant t's copy of
+// any of them is at tenant 0's pointer + t * stride() words.  Plans take tenant 0's pointers and select per instance at run time.
+class KeyBank {
+public:
+  KeyBank(std::shared_ptr<Device> dev, const std::set<u64> &elts, int capacity) : dev_(std::move(dev)), elts_(elts.begin(), elts.end()) {
+    if (capacity < 1 || capacity > 65535) throw std::invalid_argument("key bank capacity must be in [1, 65535]");
+    const std::size_t N = dev_->N(), k = (std::size_t)dev_->k();
+    if (k < 2) throw std::invalid_argument("a key bank needs at least two primes");
+    keyWords_ = (k - 1) * 2 * k * N;
+    for (std::size_t ell = 1; ell < k; ell++) constWords_ += 2 * (ell + 1) * N;
+    stride_ = keyWords_ * (1 + elts_.size()) + constWords_ * elts_.size();
+    for (u64 e : elts_) check(evab_galois_prepare(dev_->ctx(), e));
+    bank_ = DBuf(dev_, stride_ * (std::size_t)capacity);
+    used_.assign(capacity, 0);
+    dev_->sync();
+  }
+  int capacity() const { return (int)used_.size(); }
+  int tenants() const { return (int)std::count(used_.begin(), used_.end(), 1); }
+  std::size_t stride() const { return stride_; }                 // words
+  std::size_t keyWords() const { return keyWords_ * (1 + elts_.size()); }
+  std::size_t constWords() const { return constWords_ * elts_.size(); }
+  const std::vector<u64> &elements() const { return elts_; }
+  bool has(u64 elt) const { return std::binary_search(elts_.begin(), elts_.end(), elt); }
+  bool occupied(int t) const { return t >= 0 && t < capacity() && used_[t]; }
+  void requireOccupied(int t) const {
+    if (!occupied(t)) throw std::invalid_argument("tenant " + std::to_string(t) + " has no keys on this server");
+  }
+  // tenant 0's copies (the layout shared by every tenant)
+  const u64 *relin(int t = 0) const { return bank_.get() + (std::size_t)t * stride_; }
+  const u64 *galois(u64 elt, int t = 0) const { return relin(t) + keyWords_ * (1 + index(elt)); }
+  const u64 *hoistConst(u64 elt, int ell, int t = 0) const {
+    if (ell < 1 || ell >= dev_->k()) throw std::invalid_argument("hoist constant level out of range");
+    std::size_t off = keyWords_ * (1 + elts_.size()) + constWords_ * index(elt);
+    for (int l = 1; l < ell; l++) off += 2 * (std::size_t)(l + 1) * dev_->N();
+    return relin(t) + off;
+  }
+  // copies host images [k-1][2][k][N] (shapes checked by the caller) of the relinearization key and of a Galois key for every
+  // element into a free region and computes its hoist constants; returns the tenant id
+  int add(const u64 *relinKey, const std::map<u64, const u64 *> &galoisKeys) {
+    const auto it = std::find(used_.begin(), used_.end(), 0);
+    if (it == used_.end()) throw std::runtime_error("the key bank is full (" + std::to_string(capacity()) + " tenants): remove a tenant first");
+    const int t = (int)(it - used_.begin());
+    u64 *base = bank_.get() + (std::size_t)t * stride_;
+    dev_->upload(base, relinKey, keyWords_ * 8);
+    DBuf tmp(dev_, (std::size_t)dev_->k() * dev_->N());
+    for (u64 e : elts_) {
+      u64 *key = const_cast<u64 *>(galois(e, t));
+      dev_->upload(key, galoisKeys.at(e), keyWords_ * 8);
+      for (int ell = 1; ell < dev_->k(); ell++)
+        check(evab_rotate_hoist_const(dev_->ctx(), ell, e, key, const_cast<u64 *>(hoistConst(e, ell, t)), tmp.get(), nullptr));
+    }
+    dev_->sync();
+    used_[t] = 1;
+    return t;
+  }
+  void remove(int t) { requireOccupied(t); used_[t] = 0; }
+
+private:
+  std::size_t index(u64 elt) const {
+    auto it = std::lower_bound(elts_.begin(), elts_.end(), elt);
+    if (it == elts_.end() || *it != elt) throw std::invalid_argument("Galois key not present");
+    return (std::size_t)(it - elts_.begin());
+  }
+  std::shared_ptr<Device> dev_;
+  std::vector<u64> elts_;                 // sorted
+  std::size_t keyWords_ = 0, constWords_ = 0, stride_ = 0;   // one key; the constants of one element; one tenant
+  std::vector<char> used_;
+  DBuf bank_;
+};
 
 class Executor {
 public:
-  Executor(std::shared_ptr<Device> dev, const KeySet &keys, Program &program, ExecOptions opt = {})
-      : dev_(std::move(dev)), keys_(keys), prog_(program), plan_(plan(opt)), N_(dev_->N()) {
+  // bank != null: keys come from the bank, tenant per instance (setTenants); `keys` is not read.  The plan is the same either way.
+  Executor(std::shared_ptr<Device> dev, const KeySet &keys, Program &program, ExecOptions opt = {}, const KeyBank *bank = nullptr)
+      : dev_(std::move(dev)), keys_(keys), bank_(bank), prog_(program), plan_(plan(opt)), N_(dev_->N()) {
     materialise();
   }
   ~Executor() {
     if (graph_) evab_graph_destroy(dev_->ctx(), graph_);
     if (hostFlags_) evab_host_free(hostFlags_);
+    if (tenantHost_) evab_host_free(tenantHost_);
     for (void *e : events_) evab_event_destroy(dev_->ctx(), e);
     for (void *s : streams_) evab_stream_destroy(dev_->ctx(), s);
   }
@@ -61,8 +140,15 @@ public:
   // device-resident run: inputs must already be in valuePtr(input term); raw
   // inputs set through setRawInput.  Enqueues the whole program on `stream`
   // (graph launch or multi-stream replay); does not synchronise.
+  // the tenant of every instance of the next runs (bank-bound executors).  The page-locked copy is read by run()'s stream-ordered
+  // upload: callers rewrite it only once the previous run's stream has been synchronised
+  void setTenants(const int *tenants, int n) {
+    if (!bank_ || n != plan_.opt.batch) throw std::logic_error("setTenants: one tenant per instance of a bank-bound plan");
+    for (int b = 0; b < n; b++) tenantHost_[b] = tenants[b];
+  }
   void run(void *stream) {
     if (rawDirty_) { evalRawAndEncodes(stream); rawDirty_ = false; }
+    if (bank_) dev_->upload(tenantDev_.get(), tenantHost_, 4 * (std::size_t)plan_.opt.batch, stream);   // read by the kernels, not baked into the graph
     if (plan_.opt.useGraph && verbosity() < 2) {   // debug verbosity: step-by-step replay so that every term is reported
       if (!graph_ || !graphValid_) capture();
       check(evab_graph_launch(dev_->ctx(), graph_, stream));
@@ -118,22 +204,32 @@ private:
     // plan-time constants: raw values and (optionally) their encodings
     evalRawAndEncodes(nullptr);
     rawDirty_ = false;
-    // Galois tables of every rotation; for each (element, ell) a shared mod-up serves, its key-dependent constant
+    // Galois tables of every rotation; for each (element, ell) a shared mod-up serves, its key-dependent constant (a key bank
+    // holds those of every tenant)
     std::set<std::pair<u64, int>> done;   // ell 0: Galois table only
     p.forEachRotation([&](const Term *r, bool hoisted) {
       const u64 elt = galoisElt(*r);
-      if (!keys_.galois.count(elt)) throw std::invalid_argument("Galois key not present");
+      if (!(bank_ ? bank_->has(elt) : keys_.galois.count(elt) > 0)) throw std::invalid_argument("Galois key not present");
       const int ell = hoisted ? p.vals[r->index].ell : 0;
       if (!done.emplace(elt, ell).second) return;
       check(evab_galois_prepare(dev_->ctx(), elt));
-      if (!ell) return;
+      if (!ell || bank_) return;
       DBuf cadd(dev_, evab_hoist_const_bytes(dev_->ctx(), ell) / 8), tmp(dev_, (std::size_t)(ell + 1) * N_);
       check(evab_rotate_hoist_const(dev_->ctx(), ell, elt, keys_.galois.at(elt).get(), cadd.get(), tmp.get(), nullptr));
       dev_->sync();
       hoistConst_.emplace(std::make_pair(elt, ell), std::move(cadd));
     });
     if (p.numFlags) check(evab_host_alloc(8 * p.numFlags * 8 * (std::size_t)B, (void **)&hostFlags_));
+    if (bank_) {
+      tenantDev_ = DBuf(dev_, ((std::size_t)B + 1) / 2);
+      check(evab_host_alloc(4 * (std::size_t)B, (void **)&tenantHost_));
+      std::fill(tenantHost_, tenantHost_ + B, 0);
+      dev_->sync();
+    }
   }
+  const u64 *relinKey() const { return bank_ ? bank_->relin() : keys_.relin.get(); }
+  const u64 *galoisKey(u64 elt) const { return bank_ ? bank_->galois(elt) : keys_.galois.at(elt).get(); }
+  const u64 *hoistConst(u64 elt, int ell) const { return bank_ ? bank_->hoistConst(elt, ell) : hoistConst_.at(std::make_pair(elt, ell)).get(); }
   u64 galoisElt(const Term &t) const {
     const int steps = t.op == Op::RotateLeftConst ? *t.rotation : -*t.rotation;
     const u64 elt = evab_galois_elt_from_step(N_, steps);
@@ -249,8 +345,8 @@ private:
     auto hoisted = [&](const std::vector<const Term *> &rots, int ell) {
       for (const Term *r : rots) {
         const u64 elt = galoisElt(*r);
-        elts.push_back(elt); keys.push_back(keys_.galois.at(elt).get());
-        cadds.push_back(hoistConst_.at(std::make_pair(elt, ell)).get());
+        elts.push_back(elt); keys.push_back(galoisKey(elt));
+        cadds.push_back(hoistConst(elt, ell));
       }
     };
     switch (st.kind) {
@@ -329,13 +425,12 @@ private:
         else {
           const u64 elt = galoisElt(t);
           if (st.hoist >= 0 && p.opt.hoistModUp)
-            check(evab_rotate_modup_prepared(c, o.ell, out, P(0), A + p.hoistExtOff[st.hoist], elt, keys_.galois.at(elt).get(),
-                                             hoistConst_.at(std::make_pair(elt, o.ell)).get(), work, stream));
-          else if (st.hoist >= 0) check(evab_rotate_prepared(c, o.ell, out, P(0), A + p.hoistOff[st.hoist], elt, keys_.galois.at(elt).get(), work, stream));
-          else check(evab_rotate(c, o.ell, out, P(0), elt, keys_.galois.at(elt).get(), work, stream));
+            check(evab_rotate_modup_prepared(c, o.ell, out, P(0), A + p.hoistExtOff[st.hoist], elt, galoisKey(elt), hoistConst(elt, o.ell), work, stream));
+          else if (st.hoist >= 0) check(evab_rotate_prepared(c, o.ell, out, P(0), A + p.hoistOff[st.hoist], elt, galoisKey(elt), work, stream));
+          else check(evab_rotate(c, o.ell, out, P(0), elt, galoisKey(elt), work, stream));
         }
         break;
-      case Op::Relinearize: check(evab_relinearize(c, o.ell, out, P(0), keys_.relin.get(), work, stream)); break;
+      case Op::Relinearize: check(evab_relinearize(c, o.ell, out, P(0), relinKey(), work, stream)); break;
       case Op::ModSwitch: check(evab_mod_switch(c, V(0).ell, out, P(0), V(0).size, stream)); break;
       case Op::Rescale: check(evab_rescale(c, V(0).ell, out, P(0), V(0).size, work, stream)); break;
       default: throw std::runtime_error(std::string("Unhandled op ") + opName(t.op));
@@ -346,6 +441,7 @@ private:
     const Plan &p = plan_;
     evab_ctx *c = dev_->ctx();
     BatchGuard bg(p.opt.batch, p.stride, p.rawStride);
+    KeyBankGuard kg(bank_ ? reinterpret_cast<const std::int32_t *>(tenantDev_.get()) : nullptr, bank_ ? bank_->stride() : 0);
     void *forkEv = events_[p.numEvents + p.usedStreams];
     for (int b = 0; p.numFlags && b < p.opt.batch; b++)   // zero-coefficient flags of the shared mod-ups
       check(evab_memset_zero(c, arena_.get() + (std::size_t)b * p.stride + p.flagsOff, 8 * p.numFlags * 8, stream));
@@ -374,12 +470,15 @@ private:
 
   std::shared_ptr<Device> dev_;
   const KeySet &keys_;
+  const KeyBank *bank_;
   Program &prog_;
   Plan plan_;
   u64 N_;
   std::vector<std::vector<std::vector<double>>> rawsB_;   // [instance][term]
   std::map<std::pair<u64, int>, DBuf> hoistConst_;        // (galois element, ell) -> cadd [2][ell+1][N]
   u64 *hostFlags_ = nullptr;                              // page-locked copy of the flags of the last run
+  DBuf tenantDev_;                                        // bank-bound: int32 tenant of every instance, read by the kernels
+  std::int32_t *tenantHost_ = nullptr;                    // its page-locked source (setTenants)
   std::unordered_set<std::uint64_t> rawUploaded_;
   bool staticEncoded_ = false;
   DBuf rawArena_;

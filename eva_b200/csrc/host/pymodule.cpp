@@ -28,6 +28,7 @@ static void requireShape(const u64arr &a, std::initializer_list<std::size_t> sha
 
 // set_options: one argument list for B200Public and for the planner test hook (_plan), which parses its options dict through it
 static ExecOptions &optionsOf(B200Public &p) { return p.options; }
+static ExecOptions &optionsOf(B200Server &s) { return s.pub().options; }
 static ExecOptions &optionsOf(ExecOptions &o) { return o; }
 template <class Self>
 static void setOptions(Self &self, int streams, bool graph, bool cache, bool dedup, int fuse, bool fuseSums, bool hoist, bool uniformEncode, bool dedupTerms,
@@ -56,6 +57,24 @@ struct PyPending {
   py::object program, inputs;
   ~PyPending() { batch.reset(); }
 };
+
+// test hook shared by B200Public and B200Server: the value of a term in instance b of a plan's arena
+static py::object debugValue(B200Public &p, Program &prog, std::uint64_t index, int batch, int b) {
+  Executor &ex = p.executorFor(prog, batch);
+  const ValueInfo &vi = ex.info(index);
+  auto dev = p.shared()->dev;
+  if (vi.kind == Kind::Raw) return py::cast(ex.rawValue(index, b));
+  if (vi.kind == Kind::None || vi.fused) return py::none();   // fused away: never materialised
+  if (!ex.intact(index))
+    throw std::runtime_error("term " + std::to_string(index) + " is not kept by this plan's packed arena (its storage is reused after its last "
+                             "use); only inputs, outputs and cached constants can be read back");
+  const std::size_t polys = vi.kind == Kind::Cipher ? vi.size : 1;
+  u64arr a({polys, (std::size_t)vi.ell, (std::size_t)dev->N()});
+  dev->sync();
+  dev->download(a.mutable_data(), ex.valuePtr(index, b), a.size() * 8);
+  dev->sync();
+  return py::make_tuple(a, vi.scale);
+}
 
 PYBIND11_MODULE(_eva_b200, m) {
   m.doc() = "H100-native (sm_90a) EVA backend";
@@ -321,22 +340,7 @@ PYBIND11_MODULE(_eva_b200, m) {
         return out;
       }, py::arg("program"), py::arg("stream"), py::arg("replica") = 0, py::call_guard<py::gil_scoped_release>())
       // ---- test hooks
-      .def("debug_value", [](B200Public &p, Program &prog, std::uint64_t index, int batch, int b) -> py::object {
-        Executor &ex = p.executorFor(prog, batch);
-        const ValueInfo &vi = ex.info(index);
-        auto dev = p.shared()->dev;
-        if (vi.kind == Kind::Raw) return py::cast(ex.rawValue(index, b));
-        if (vi.kind == Kind::None || vi.fused) return py::none();   // fused away: never materialised
-        if (!ex.intact(index))
-          throw std::runtime_error("term " + std::to_string(index) + " is not kept by this plan's packed arena (its storage is reused after its last "
-                                   "use); only inputs, outputs and cached constants can be read back");
-        const std::size_t polys = vi.kind == Kind::Cipher ? vi.size : 1;
-        u64arr a({polys, (std::size_t)vi.ell, (std::size_t)dev->N()});
-        dev->sync();
-        dev->download(a.mutable_data(), ex.valuePtr(index, b), a.size() * 8);
-        dev->sync();
-        return py::make_tuple(a, vi.scale);
-      }, py::arg("program"), py::arg("index"), py::arg("batch") = 1, py::arg("instance") = 0)
+      .def("debug_value", &debugValue, py::arg("program"), py::arg("index"), py::arg("batch") = 1, py::arg("instance") = 0)
       .def("encode", [](B200Public &p, const std::vector<double> &values, double scale, int ell, bool host) {
         auto dev = p.shared()->dev;
         DBuf pt(dev, (std::size_t)ell * dev->N());
@@ -403,6 +407,100 @@ PYBIND11_MODULE(_eva_b200, m) {
         d["secret_key"] = a;
         return d;
       });
+
+  // ---- multi-tenant serving: one device, one parameter set, the evaluation keys of many clients in a key bank
+  typedef std::vector<std::pair<int, const B200Valuation *>> Requests;
+  py::class_<B200Server> srv(mb, "B200Server",
+                             "Executes compiled programs for many clients: each client's evaluation keys are a tenant of a key bank of fixed "
+                             "capacity, the plans are shared by all tenants, and every instance of a batch runs with its own tenant's keys");
+  srv.def(py::init<const CKKSParameters &, int, int>(), py::arg("params"), py::arg("capacity") = 64, py::arg("device") = 0)
+      .def("add_raw_keys", [](B200Server &s, const u64arr &relin, const std::map<u64, u64arr> &galois) {
+        const std::size_t kk = s.shared()->dev->k(), N = s.shared()->dev->N();
+        requireShape(relin, {kk - 1, 2, kk, N}, "relinearization key");
+        std::map<u64, const u64 *> g;   // the elements of the rotation set (addKeys reports a missing one)
+        for (u64 e : s.bank().elements())
+          if (auto it = galois.find(e); it != galois.end()) {
+            requireShape(it->second, {kk - 1, 2, kk, N}, "Galois key");
+            g[e] = it->second.data();
+          }
+        py::gil_scoped_release rel;
+        return s.addKeys(relin.data(), g);
+      }, py::arg("relin_key"), py::arg("galois_keys"), "copy a client's relinearization key and Galois keys (host arrays [k-1][2][k][N]) into a "
+         "free tenant slot and compute its hoist constants; returns the tenant id")
+      .def("add_keys", [](B200Server &s, B200Public &p) {
+        auto src = p.shared();
+        if (src->dev->N() != s.shared()->dev->N() || src->dev->primes() != s.shared()->dev->primes())
+          throw std::invalid_argument("the context's N / primes do not match the server's");
+        const std::size_t kk = s.shared()->dev->k(), words = (kk - 1) * 2 * kk * s.shared()->dev->N();
+        if (!src->keys.relin || src->keys.relin.words() != words) throw std::invalid_argument("the context has no relinearization key of the server's shape");
+        std::vector<u64> relin(words);
+        std::map<u64, std::vector<u64>> gal;
+        std::map<u64, const u64 *> g;
+        src->dev->sync();
+        src->dev->download(relin.data(), src->keys.relin.get(), words * 8);
+        for (u64 e : s.bank().elements()) {
+          auto it = src->keys.galois.find(e);
+          if (it == src->keys.galois.end()) continue;   // addKeys reports it
+          if (it->second.words() != words) throw std::invalid_argument("Galois key does not match the server's shape");
+          auto &h = gal[e];
+          h.resize(words);
+          src->dev->download(h.data(), it->second.get(), words * 8);
+          g[e] = h.data();
+        }
+        src->dev->sync();
+        py::gil_scoped_release rel;
+        return s.addKeys(relin.data(), g);
+      }, py::arg("public_context"), "add_raw_keys with the evaluation keys of a client's B200Public (same N and primes)")
+      .def("remove_keys", &B200Server::removeKeys, py::arg("tenant"))
+      .def("execute", [](B200Server &s, Program &prog, int tenant, const B200Valuation &in) {
+        return std::move(s.executeBatch(prog, {{tenant, &in}})[0]);
+      }, py::arg("program"), py::arg("tenant"), py::arg("inputs"), py::call_guard<py::gil_scoped_release>())
+      .def("execute_batch", &B200Server::executeBatch, py::arg("program"), py::arg("requests"), py::call_guard<py::gil_scoped_release>(),
+           "requests: [(tenant, valuation), ...]; returns a list of valuations")
+      .def("execute_batch_async", [](B200Server &s, py::object program, py::list requests, int slot) {
+        Program &prog = program.cast<Program &>();
+        Requests rq = requests.cast<Requests>();
+        auto out = std::make_shared<PyPending>();
+        { py::gil_scoped_release rel; out->batch = s.submit(prog, rq, slot); }
+        out->program = program; out->inputs = requests;
+        return out;
+      }, py::arg("program"), py::arg("requests"), py::arg("slot") = 0)
+      .def("execute_batch_result", [](B200Server &s, std::shared_ptr<PyPending> h) {
+        std::vector<B200Valuation> outs;
+        { py::gil_scoped_release rel; outs = s.pub().collect(*h->batch); }
+        return outs;
+      }, py::arg("handle"))
+      .def("drop_plan", [](B200Server &s, Program &prog, int batch, int replica) { s.pub().dropExecutor(prog, batch, replica); },
+           py::arg("program"), py::arg("batch") = 1, py::arg("replica") = 0)
+      .def("plan_stats", [](B200Server &s, Program &prog, int batch, int replica) { return s.pub().executorFor(prog, batch, replica).planStats(); },
+           py::arg("program"), py::arg("batch") = 1, py::arg("replica") = 0)
+      .def("plans_built", [](B200Server &s) { return s.pub().plansBuilt; }, "plans built so far (each: plan, arena, graph capture)")
+      .def("launch_count", [](B200Server &s) { return evab_launch_count(s.shared()->dev->ctx()); })
+      .def("bank_info", [](B200Server &s) {
+        const KeyBank &b = s.bank();
+        std::lock_guard<std::mutex> guard(s.shared()->execMutex);   // add / remove change the occupancy under it
+        py::dict d;
+        d["capacity"] = b.capacity(); d["tenants"] = b.tenants(); d["galois_elements"] = b.elements();
+        d["tenant_bytes"] = b.stride() * 8; d["key_bytes_per_tenant"] = b.keyWords() * 8; d["hoist_const_bytes_per_tenant"] = b.constWords() * 8;
+        d["bank_bytes"] = b.stride() * 8 * (std::size_t)b.capacity();
+        return d;
+      })
+      .def("primes", [](B200Server &s) { return s.shared()->dev->primes(); })
+      // ---- benchmark hooks (as B200Public's): device-resident execution of requests staged on a plan replica
+      .def("stage_inputs", [](B200Server &s, Program &prog, const Requests &rq, std::uintptr_t stream, int replica) {
+        std::vector<int> tenants;
+        for (auto &r : rq) tenants.push_back(r.first);
+        std::lock_guard<std::mutex> guard(s.shared()->execMutex);
+        for (int t : tenants) s.bank().requireOccupied(t);
+        Executor &ex = s.pub().executorFor(prog, (int)rq.size(), replica);
+        ex.setTenants(tenants.data(), (int)tenants.size());
+        for (std::size_t b = 0; b < rq.size(); b++) s.pub().stageInputs(ex, prog, *rq[b].second, (void *)stream, (int)b);
+      }, py::arg("program"), py::arg("requests"), py::arg("stream"), py::arg("replica") = 0)
+      .def("run_resident", [](B200Server &s, Program &prog, std::uintptr_t stream, int batch, int replica) { s.pub().executorFor(prog, batch, replica).run((void *)stream); },
+           py::arg("program"), py::arg("stream"), py::arg("batch") = 1, py::arg("replica") = 0, py::call_guard<py::gil_scoped_release>())
+      .def("debug_value", [](B200Server &s, Program &prog, std::uint64_t index, int batch, int b) { return debugValue(s.pub(), prog, index, batch, b); },
+           py::arg("program"), py::arg("index"), py::arg("batch") = 1, py::arg("instance") = 0);
+  defSetOptions(srv);
 
   mb.def("generate_keys", [](const CKKSParameters &p, int device, std::uint64_t seed) { return generateKeys(p, device, seed); },
          py::arg("abstract_params"), py::arg("device") = 0, py::arg("seed") = 0);

@@ -360,18 +360,24 @@ int rotate_modup_many_impl(BE &be, const CtxView &c, int ell, int n, u64 *out, c
 inline size_t rotate_wsum_work_elems(const CtxView &c, int ell, int n, int nout) {
   return (size_t)2 * n * 2 * c.N + (size_t)2 * nout * 2 * ell * c.N;
 }
+#if !defined(__CUDACC__)
+// key-bank offset of a replayed instance: the replay backend's key_off() where it has one (evab_set_key_bank), else 0
+template <class BE> auto replay_key_off(BE &be, int) -> decltype(be.key_off()) { return be.key_off(); }
+template <class BE> long long replay_key_off(BE &, long) { return 0; }
+#endif
 // the inner products with the weighting: k_rot_wsum_ip in the CUDA build; compiled without CUDA (the CPU emulator of the tests) the
 // same element body replayed serially on the host
 template <class BE> int rot_wsum_ip_step(BE &be, const WsumIpArgs &A) {
 #if defined(__CUDACC__)
   return be.rot_wsum_ip(A);
 #else
+  const long long koff = replay_key_off(be, 0);
   for (int mi = 0; mi <= A.ell; mi++)
     for (int j = 0; j < A.N; j += 2) switch (A.nout) {
-        case 1: rot_wsum_ip_elem<1>(A, mi, j); break;
-        case 2: rot_wsum_ip_elem<2>(A, mi, j); break;
-        case 3: rot_wsum_ip_elem<3>(A, mi, j); break;
-        case 4: rot_wsum_ip_elem<4>(A, mi, j); break;
+        case 1: rot_wsum_ip_elem<1>(A, mi, j, 0, koff); break;
+        case 2: rot_wsum_ip_elem<2>(A, mi, j, 0, koff); break;
+        case 3: rot_wsum_ip_elem<3>(A, mi, j, 0, koff); break;
+        case 4: rot_wsum_ip_elem<4>(A, mi, j, 0, koff); break;
         default: return be.error("rotate_wsum: 1..4 output sums");
       }
   return 0;

@@ -169,8 +169,9 @@ struct IpArgs {
   const u64 *cadd;
   int ell, k, N;
 };
-// off: batch instance offset (words) of t / ext / acc (the key is shared by all instances)
-EVAB_HD void ks_inner_elem(const IpArgs &A, int mi, int j, long long off = 0) {
+// off: batch instance offset (words) of t / ext / acc; koff: key offset (words) of the instance's tenant in a key bank
+// (evab_set_key_bank), applied to key and cadd; 0 when all instances share the key
+EVAB_HD void ks_inner_elem(const IpArgs &A, int mi, int j, long long off = 0, long long koff = 0) {
   const int row = (mi == A.ell) ? A.k - 1 : mi;
   const PrimeDev P = A.primes[row];
   const size_t N = A.N;
@@ -186,8 +187,8 @@ EVAB_HD void ks_inner_elem(const IpArgs &A, int mi, int j, long long off = 0) {
       if (A.eperm) { v.x = EVAB_LDG(ep + EVAB_LDG(A.eperm + j)); v.y = EVAB_LDG(ep + EVAB_LDG(A.eperm + j + 1)); }
       else v = ld2(ep + j);
     }
-    const u64x2 k0 = ld2(A.key + (((size_t)J * 2 + 0) * A.k + row) * N + j);
-    const u64x2 k1 = ld2(A.key + (((size_t)J * 2 + 1) * A.k + row) * N + j);
+    const u64x2 k0 = ld2(A.key + koff + (((size_t)J * 2 + 0) * A.k + row) * N + j);
+    const u64x2 k1 = ld2(A.key + koff + (((size_t)J * 2 + 1) * A.k + row) * N + j);
     mac128(l0x, h0x, v.x, k0.x); mac128(l0y, h0y, v.y, k0.y);
     mac128(l1x, h1x, v.x, k1.x); mac128(l1y, h1y, v.y, k1.y);
   }
@@ -196,7 +197,7 @@ EVAB_HD void ks_inner_elem(const IpArgs &A, int mi, int j, long long off = 0) {
   r0.x = reduce128(l0x, h0x, P); r0.y = reduce128(l0y, h0y, P);
   r1.x = reduce128(l1x, h1x, P); r1.y = reduce128(l1y, h1y, P);
   if (A.cadd) {
-    const u64x2 c0 = ld2(A.cadd + ((size_t)0 * (A.ell + 1) + mi) * N + j), c1 = ld2(A.cadd + ((size_t)1 * (A.ell + 1) + mi) * N + j);
+    const u64x2 c0 = ld2(A.cadd + koff + ((size_t)0 * (A.ell + 1) + mi) * N + j), c1 = ld2(A.cadd + koff + ((size_t)1 * (A.ell + 1) + mi) * N + j);
     r0.x = addmod(r0.x, c0.x, P.p); r0.y = addmod(r0.y, c0.y, P.p);
     r1.x = addmod(r1.x, c1.x, P.p); r1.y = addmod(r1.y, c1.y, P.p);
   }
@@ -223,7 +224,8 @@ struct RotManyArgs {
   const PrimeDev *primes;
   int n, ell, k, N;
 };
-EVAB_HD void rot_many_elem(const RotManyArgs &A, int i, int mi, int j, long long off = 0) {
+// koff: key offset of the instance's tenant (ks_inner_elem), applied to key[i] and cadd[i]
+EVAB_HD void rot_many_elem(const RotManyArgs &A, int i, int mi, int j, long long off = 0, long long koff = 0) {
   const int row = (mi == A.ell) ? A.k - 1 : mi;
   const PrimeDev P = A.primes[row];
   const size_t N = A.N;
@@ -232,12 +234,12 @@ EVAB_HD void rot_many_elem(const RotManyArgs &A, int i, int mi, int j, long long
   for (int J = 0; J < A.ell; J++) {
     const u64 *src = (row == J) ? A.t + off + (size_t)J * N : A.ext + off + ((size_t)mi * A.ell + J) * N;
     const u64 vx = EVAB_LDG(src + pj0), vy = EVAB_LDG(src + pj1);
-    const u64x2 k0 = ld2(A.key[i] + (((size_t)J * 2 + 0) * A.k + row) * N + j);
-    const u64x2 k1 = ld2(A.key[i] + (((size_t)J * 2 + 1) * A.k + row) * N + j);
+    const u64x2 k0 = ld2(A.key[i] + koff + (((size_t)J * 2 + 0) * A.k + row) * N + j);
+    const u64x2 k1 = ld2(A.key[i] + koff + (((size_t)J * 2 + 1) * A.k + row) * N + j);
     mac128(l0x, h0x, vx, k0.x); mac128(l0y, h0y, vy, k0.y);
     mac128(l1x, h1x, vx, k1.x); mac128(l1y, h1y, vy, k1.y);
   }
-  const u64x2 c0 = ld2(A.cadd[i] + ((size_t)0 * (A.ell + 1) + mi) * N + j), c1 = ld2(A.cadd[i] + ((size_t)1 * (A.ell + 1) + mi) * N + j);
+  const u64x2 c0 = ld2(A.cadd[i] + koff + ((size_t)0 * (A.ell + 1) + mi) * N + j), c1 = ld2(A.cadd[i] + koff + ((size_t)1 * (A.ell + 1) + mi) * N + j);
   u64x2 r0, r1;
   r0.x = addmod(reduce128(l0x, h0x, P), c0.x, P.p); r0.y = addmod(reduce128(l0y, h0y, P), c0.y, P.p);
   r1.x = addmod(reduce128(l1x, h1x, P), c1.x, P.p); r1.y = addmod(reduce128(l1y, h1y, P), c1.y, P.p);
@@ -310,7 +312,8 @@ struct WsumIpArgs {
 // coefficients j, j+1 of row mi (q_0 .. q_{ell-1}, P) of both polynomials, every rotation and every output (nout == NOUT).  acc_i is
 // rot_many_elem's canonical value: the inner product through perm_i + cadd_i, and on a q row + perm_i(P c0) = (P mod q_m) c0[perm_i(j)],
 // read from c0 directly.  A P row is stored; a q row is weighted into A, which then takes the taps.
-template <int NOUT> EVAB_HD void rot_wsum_ip_elem(const WsumIpArgs &A, int mi, int j, long long off = 0) {
+// koff: key offset of the instance's tenant (ks_inner_elem), applied to key[i] and cadd[i]
+template <int NOUT> EVAB_HD void rot_wsum_ip_elem(const WsumIpArgs &A, int mi, int j, long long off = 0, long long koff = 0) {
   const bool qrow = mi < A.ell;
   const int row = qrow ? mi : A.k - 1;
   const PrimeDev P = A.primes[row];
@@ -330,12 +333,12 @@ template <int NOUT> EVAB_HD void rot_wsum_ip_elem(const WsumIpArgs &A, int mi, i
     for (int J = 0; J < A.ell; J++) {
       const u64 *src = (row == J) ? A.t + off + (size_t)J * N : A.ext + off + ((size_t)mi * A.ell + J) * N;
       const u64 vx = EVAB_LDG(src + p0), vy = EVAB_LDG(src + p1);
-      const u64x2 k0 = ld2(A.key[i] + (((size_t)J * 2 + 0) * A.k + row) * N + j);
-      const u64x2 k1 = ld2(A.key[i] + (((size_t)J * 2 + 1) * A.k + row) * N + j);
+      const u64x2 k0 = ld2(A.key[i] + koff + (((size_t)J * 2 + 0) * A.k + row) * N + j);
+      const u64x2 k1 = ld2(A.key[i] + koff + (((size_t)J * 2 + 1) * A.k + row) * N + j);
       mac128(l0x, h0x, vx, k0.x); mac128(l0y, h0y, vy, k0.y);
       mac128(l1x, h1x, vx, k1.x); mac128(l1y, h1y, vy, k1.y);
     }
-    const u64x2 c0 = ld2(A.cadd[i] + ((size_t)0 * (A.ell + 1) + mi) * N + j), c1 = ld2(A.cadd[i] + ((size_t)1 * (A.ell + 1) + mi) * N + j);
+    const u64x2 c0 = ld2(A.cadd[i] + koff + ((size_t)0 * (A.ell + 1) + mi) * N + j), c1 = ld2(A.cadd[i] + koff + ((size_t)1 * (A.ell + 1) + mi) * N + j);
     u64x2 r0, r1;
     r0.x = addmod(reduce128(l0x, h0x, P), c0.x, P.p); r0.y = addmod(reduce128(l0y, h0y, P), c0.y, P.p);
     r1.x = addmod(reduce128(l1x, h1x, P), c1.x, P.p); r1.y = addmod(reduce128(l1y, h1y, P), c1.y, P.p);
@@ -430,7 +433,8 @@ struct LazyRotSumArgs {
 // One rotation's share at elements (j, j+1) of row mi, for every output sum it takes part in.  The key-switch inner product of
 // the rotation is computed once and weighted per output; every value is reduced below p, so that up to LRS_MAX of them add up
 // inside 64 bits.  part[o] = { w.(ip0+cadd0) + P.w.perm(c0), w.(ip1+cadd1) } for x and y.
-EVAB_HD void lazy_rotsum_part(const LazyRotSumArgs &A, int mi, int j, int i, long long off, u64 part[LRS_OUT][4]) {
+// koff: key offset of the instance's tenant (ks_inner_elem), applied to key[i] and cadd[i]
+EVAB_HD void lazy_rotsum_part(const LazyRotSumArgs &A, int mi, int j, int i, long long off, u64 part[LRS_OUT][4], long long koff = 0) {
   const int row = (mi == A.ell) ? A.k - 1 : mi;
   const PrimeDev P = A.primes[row];
   const size_t N = A.N;
@@ -440,12 +444,12 @@ EVAB_HD void lazy_rotsum_part(const LazyRotSumArgs &A, int mi, int j, int i, lon
   for (int J = 0; J < A.ell; J++) {
     const u64 *src = (row == J) ? A.t + off + (size_t)J * N : A.ext + off + ((size_t)mi * A.ell + J) * N;
     const u64 vx = EVAB_LDG(src + pj0), vy = EVAB_LDG(src + pj1);
-    const u64x2 k0 = ld2(A.key[i] + (((size_t)J * 2 + 0) * A.k + row) * N + j);
-    const u64x2 k1 = ld2(A.key[i] + (((size_t)J * 2 + 1) * A.k + row) * N + j);
+    const u64x2 k0 = ld2(A.key[i] + koff + (((size_t)J * 2 + 0) * A.k + row) * N + j);
+    const u64x2 k1 = ld2(A.key[i] + koff + (((size_t)J * 2 + 1) * A.k + row) * N + j);
     mac128(l0x, h0x, vx, k0.x); mac128(l0y, h0y, vy, k0.y);
     mac128(l1x, h1x, vx, k1.x); mac128(l1y, h1y, vy, k1.y);
   }
-  const u64x2 c0 = ld2(A.cadd[i] + ((size_t)0 * (A.ell + 1) + mi) * N + j), c1 = ld2(A.cadd[i] + ((size_t)1 * (A.ell + 1) + mi) * N + j);
+  const u64x2 c0 = ld2(A.cadd[i] + koff + ((size_t)0 * (A.ell + 1) + mi) * N + j), c1 = ld2(A.cadd[i] + koff + ((size_t)1 * (A.ell + 1) + mi) * N + j);
   u64 a0x = addmod(reduce128(l0x, h0x, P), c0.x, P.p), a0y = addmod(reduce128(l0y, h0y, P), c0.y, P.p);
   const u64 a1x = addmod(reduce128(l1x, h1x, P), c1.x, P.p), a1y = addmod(reduce128(l1y, h1y, P), c1.y, P.p);
   if (mi < A.ell) {   // + perm(P * c0) (the diagonal of ext): comes back as perm(c0) from the division by P

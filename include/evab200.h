@@ -83,6 +83,14 @@ int evab_graph_destroy(evab_ctx *ctx, void *graph_exec);
  * b * value_stride (doubles); keys and tables are shared.  One fat launch replaces
  * `batch` launches (horizontal fusion across program instances, SURVEY.md 8f-3). */
 int evab_set_batch(int batch, size_t stride_words, size_t value_stride);
+/* Per-instance keys (thread-local, next to evab_set_batch): until reset with NULL, every
+ * key pointer and hoist-constant pointer that the relinearize / rotate / rotate_prepared /
+ * rotate_modup_prepared / rotate_modup_many / rotate_wsum / lazy_rotsum kernels read is,
+ * for batch instance b, shifted by d_tenant_of_instance[b] * tenant_stride_words (u64
+ * words).  The caller passes tenant 0's pointers of a key bank whose tenants share one
+ * layout.  The table is device memory read when the kernels run, so a captured graph
+ * follows a table rewritten (stream-ordered) before its launch. */
+int evab_set_key_bank(const int32_t *d_tenant_of_instance, size_t tenant_stride_words);
 /* number of kernel launches issued through this context so far */
 uint64_t evab_launch_count(const evab_ctx *ctx);
 
