@@ -44,6 +44,9 @@ _SIGS = {
     "evab_hoist_const_bytes": (szt, [vp, ci]),
     "evab_rotate_modup_prepare": (ci, [vp, ci, vp, vp, vp, vp, vp]),
     "evab_rotate_hoist_const": (ci, [vp, ci, u64, vp, vp, vp, vp]),
+    "evab_hoist_const_levels_bytes": (szt, [vp]),
+    "evab_rotate_hoist_const_levels_work_bytes": (szt, [vp, ci]),
+    "evab_rotate_hoist_const_levels": (ci, [vp, ci, u64p, vp, vp, vp, vp]),
     "evab_rotate_modup_prepared": (ci, [vp, ci, vp, vp, vp, u64, vp, vp, vp, vp]),
     "evab_memset_zero": (ci, [vp, vp, szt, vp]),
     "evab_rotate_modup_scale_c0": (ci, [vp, ci, vp, vp, vp]),

@@ -256,6 +256,10 @@ template <bool BANK> __global__ void __launch_bounds__(32 * LRS_MAX) k_lazy_rots
 __global__ void __launch_bounds__(256) k_hoist_const(const HoistConstArgs A) {
   for (int j = (blockIdx.x * blockDim.x + threadIdx.x) * 2; j < A.N; j += gridDim.x * blockDim.x * 2) hoist_const_elem(A, blockIdx.y, j);
 }
+// grid (coefficient tiles, prime m, key g)
+__global__ void __launch_bounds__(256) k_hoist_const_levels(const HoistLevelsArgs A) {
+  for (int j = (blockIdx.x * blockDim.x + threadIdx.x) * 2; j < A.N; j += gridDim.x * blockDim.x * 2) hoist_levels_elem(A, blockIdx.z, blockIdx.y, j);
+}
 __global__ void __launch_bounds__(256) k_hoist_indicator(u64 *out, const u32 *ctab, int N) {
   for (int j = blockIdx.x * blockDim.x + threadIdx.x; j < N; j += gridDim.x * blockDim.x) hoist_indicator_elem(out, ctab, N, blockIdx.y, j);
 }
@@ -513,6 +517,13 @@ struct CudaBE {
   int hoist_const(const HoistConstArgs &A) {
     count();
     k_hoist_const<<<dim3((A.N / 2 + 255) / 256, A.ell + 1), 256, 0, st>>>(A);
+    CUDA_OK(cudaGetLastError());
+    return 0;
+  }
+  int hoist_levels(const HoistLevelsArgs &A, int n) {
+    if (n > 65535) return fail("hoist constants: at most 65535 keys per call");
+    count();
+    k_hoist_const_levels<<<dim3((A.N / 2 + 255) / 256, A.k, n), 256, 0, st>>>(A);
     CUDA_OK(cudaGetLastError());
     return 0;
   }
@@ -865,6 +876,18 @@ extern "C" int evab_rotate_hoist_const(evab_ctx *c, int ell, uint64_t elt, const
   u32 *perm = nullptr, *ctab = nullptr;
   if (galois_tables(c, elt, &perm, &ctab, "evab_rotate_hoist_const")) return 1;
   BE_BEGIN return hoist_const_impl(be, c->v, ell, ctab, key, out, tmp);
+}
+extern "C" size_t evab_hoist_const_levels_bytes(const evab_ctx *c) { return hoist_levels_words(c->v.k, c->v.N) * sizeof(u64); }
+extern "C" size_t evab_rotate_hoist_const_levels_work_bytes(const evab_ctx *c, int n) { return hoist_const_levels_work_elems(c->v, n) * sizeof(u64); }
+extern "C" int evab_rotate_hoist_const_levels(evab_ctx *c, int n, const uint64_t *elts, const uint64_t *keys, uint64_t *out, uint64_t *tmp, void *stream) {
+  if (n < 1) return fail("evab_rotate_hoist_const_levels: n must be >= 1");
+  std::vector<const u32 *> ctabs(n);
+  for (int g = 0; g < n; g++) {
+    u32 *perm = nullptr, *ctab = nullptr;
+    if (galois_tables(c, elts[g], &perm, &ctab, "evab_rotate_hoist_const_levels")) return 1;
+    ctabs[g] = ctab;
+  }
+  BE_BEGIN return hoist_const_levels_impl(be, c->v, n, ctabs.data(), keys, out, tmp);
 }
 extern "C" int evab_rotate_modup_prepared(evab_ctx *c, int ell, uint64_t *o, const uint64_t *a, const uint64_t *ext, uint64_t elt, const uint64_t *key,
                                           const uint64_t *cadd, void *work, void *stream) {

@@ -7,6 +7,7 @@
 #include <cstdio>
 #include <cstdlib>
 #include "executor.hpp"
+#include "slot_cache.hpp"
 #include <atomic>
 #include <mutex>
 #include <tuple>
@@ -49,12 +50,101 @@ public:
   std::map<std::string, SchemeValue> values;
 };
 
+// Paging of evaluation keys (B200Server with more tenants than key-bank regions): every registered tenant's keys live in a
+// page-locked host block, and the bank's regions are device slots holding the keys of the tenants used recently (SlotCache).
+// A batch's missing tenants are filled on the pager's own stream: a fill waits for the runs that may still read its slot (one
+// reader event per slot and replica stream), uploads the keys, recomputes the slot's hoist constants and records the slot's fill
+// event, which every run that reads the slot waits for.  The host never blocks on the way.
+class KeyPager {
+public:
+  KeyPager(std::shared_ptr<Device> dev, KeyBank &bank, int maxTenants)
+      : dev_(std::move(dev)), bank_(bank), cache_(bank.capacity()), host_(maxTenants, nullptr), fillEv_(bank.capacity(), nullptr), readers_(bank.capacity()) {
+    check(evab_stream_create(dev_->ctx(), &stream_));
+  }
+  ~KeyPager() {
+    evab_ctx *c = dev_->ctx();
+    evab_sync(c, stream_);   // fills still reading the host blocks
+    for (u64 *h : host_) if (h) evab_host_free(h);
+    for (void *e : fillEv_) if (e) evab_event_destroy(c, e);
+    for (auto &m : readers_) for (auto &r : m) evab_event_destroy(c, r.second);
+    evab_stream_destroy(c, stream_);
+  }
+  KeyPager(const KeyPager &) = delete;
+  int maxTenants() const { return (int)host_.size(); }
+  int tenants() const { return (int)std::count_if(host_.begin(), host_.end(), [](u64 *h) { return h != nullptr; }); }
+  bool registered(int t) const { return t >= 0 && t < maxTenants() && host_[t]; }
+  void requireRegistered(int t) const {
+    if (!registered(t)) throw std::invalid_argument("tenant " + std::to_string(t) + " has no keys on this server");
+  }
+  // host images [k-1][2][k][N] of the relinearization key and of every element's Galois key (checked by the caller) into a new
+  // page-locked block; no device work.  Returns the tenant id
+  int add(const u64 *relinKey, const std::map<u64, const u64 *> &galoisKeys) {
+    const auto it = std::find(host_.begin(), host_.end(), nullptr);
+    if (it == host_.end()) throw std::runtime_error("the host key store is full (" + std::to_string(maxTenants()) + " tenants): remove a tenant first");
+    const std::size_t kw = bank_.keyWords() / (1 + bank_.elements().size());
+    u64 *h = nullptr;
+    check(evab_host_alloc(bank_.keyWords() * 8, (void **)&h));
+    std::memcpy(h, relinKey, kw * 8);
+    for (std::size_t i = 0; i < bank_.elements().size(); i++) std::memcpy(h + kw * (1 + i), galoisKeys.at(bank_.elements()[i]), kw * 8);
+    *it = h;
+    return (int)(it - host_.begin());
+  }
+  void remove(int t) {
+    requireRegistered(t);
+    cache_.drop(t);
+    check(evab_sync(dev_->ctx(), stream_));   // a fill may still be reading the block
+    evab_host_free(host_[t]);
+    host_[t] = nullptr;
+  }
+  // the slot of every instance of a batch; the missing tenants' fills are enqueued on the pager's stream
+  std::vector<int> resolve(const std::vector<int> &tenants) {
+    evab_ctx *c = dev_->ctx();
+    std::vector<SlotCache::Fill> fills;
+    std::vector<int> slots = cache_.assign(tenants, fills);
+    for (auto &f : fills) {
+      for (auto &r : readers_[f.slot]) check(evab_stream_wait_event(c, stream_, r.second));
+      bank_.fill(f.slot, host_[f.tenant], stream_);
+      if (!fillEv_[f.slot]) check(evab_event_create(c, &fillEv_[f.slot]));
+      check(evab_event_record(c, fillEv_[f.slot], stream_));
+    }
+    return slots;
+  }
+  // a run on `stream` that reads `slots` waits for their fills; once enqueued, it is recorded as their reader on that stream
+  void beforeRun(void *stream, const int *slots, int n) {
+    for (int i = 0; i < n; i++)
+      if (std::find(slots, slots + i, slots[i]) == slots + i && fillEv_[slots[i]]) check(evab_stream_wait_event(dev_->ctx(), stream, fillEv_[slots[i]]));
+  }
+  void afterRun(void *stream, const int *slots, int n) {
+    for (int i = 0; i < n; i++) {
+      if (std::find(slots, slots + i, slots[i]) != slots + i) continue;
+      void *&ev = readers_[slots[i]][stream];
+      if (!ev) check(evab_event_create(dev_->ctx(), &ev));
+      check(evab_event_record(dev_->ctx(), ev, stream));
+    }
+  }
+  const SlotCache &cache() const { return cache_; }
+  std::size_t hostBytes() const { return (std::size_t)tenants() * bank_.keyWords() * 8; }
+
+private:
+  std::shared_ptr<Device> dev_;
+  KeyBank &bank_;
+  SlotCache cache_;
+  std::vector<u64 *> host_;                         // tenant -> page-locked keys (keyWords() words), null: free id
+  std::vector<void *> fillEv_;                      // slot -> event of its last fill
+  std::vector<std::map<void *, void *>> readers_;   // slot -> (replica stream -> event after its last run that read the slot)
+  void *stream_ = nullptr;                          // fills
+};
+
 struct Shared {
   std::shared_ptr<Device> dev;
   std::unique_ptr<CkksClient> client;
   KeySet keys;
   std::unique_ptr<KeyBank> bank;   // B200Server: the tenants' keys (then `keys` is empty and every batch names a tenant per instance)
+  std::unique_ptr<KeyPager> pager; // B200Server with max_tenants > capacity: tenants paged into the bank's regions
   std::mutex execMutex;   // serialises execute / executeMany callers of one context (see executeMany), and key-bank changes
+  void requireTenant(int t) const { if (pager) pager->requireRegistered(t); else bank->requireOccupied(t); }
+  // the bank region of every instance (with paging: resolved, and missing tenants' fills enqueued)
+  std::vector<int> slotsFor(const std::vector<int> &tenants) { return pager ? pager->resolve(tenants) : tenants; }
 };
 
 // the cached plan of one (program, context) pair; owned by the Program
@@ -211,7 +301,7 @@ public:
     // one caller at a time per context: plan replicas own single arenas and raw-input buffers (the reference's
     // execute is re-entrant because it builds a new executor per call; concurrent callers are serialised here)
     std::lock_guard<std::mutex> guard(s_->execMutex);
-    for (int t : tenants) s_->bank->requireOccupied(t);
+    for (int t : tenants) s_->requireTenant(t);
     if (auto prev = inFlight_[slot].lock(); prev && !prev->collected) throw std::runtime_error("slot in use: collect the batch submitted before");
     auto p = std::make_shared<PendingBatch>();
     p->program = &program; p->inputs = inputs; p->slot = slot; p->keep = s_; p->tenants = std::move(tenants);
@@ -269,6 +359,9 @@ public:
       if (const char *cap = std::getenv("EVAB_MAX_REPLICAS")) R = std::max(1, std::min(R, std::atoi(cap)));   // tests / tuning
     }
     std::vector<char> busy(R, 0);
+    // key-bank region of every instance, resolved at every enqueue (so that collect's redo refills a tenant evicted meanwhile)
+    const std::vector<int> slots = p.tenants.empty() ? std::vector<int>() : s_->slotsFor(p.tenants);
+    KeyPager *pager = s_->pager.get();
     for (int b0 = 0, g = 0; b0 < B; b0 += F, g++) {
       const int nb = std::min(F, B - b0);
       const int r = g % R;
@@ -278,13 +371,15 @@ public:
       void *st = ex.mainStream();
       if (busy[r]) s_->dev->sync(st);   // the replica's arena is reused: wait for its previous chunk
       busy[r] = 1;
-      if (!p.tenants.empty()) ex.setTenants(p.tenants.data() + b0, nb);
+      if (!slots.empty()) ex.setTenants(slots.data() + b0, nb);
       if (std::find(streams.begin(), streams.end(), st) == streams.end()) streams.push_back(st);
       if (std::find(p.plans.begin(), p.plans.end(), holder) == p.plans.end()) p.plans.push_back(holder);
       auto t1 = now();
       for (int b = 0; b < nb; b++) stageInputs(ex, program, *inputs[b0 + b], st, b);
       auto t2 = now();
+      if (pager) pager->beforeRun(st, slots.data() + b0, nb);
       ex.run(st);
+      if (pager) pager->afterRun(st, slots.data() + b0, nb);
       auto t3 = now();
       tPlan += std::chrono::duration<double>(t1 - t0).count(); tStage += std::chrono::duration<double>(t2 - t1).count();
       tRun += std::chrono::duration<double>(t3 - t2).count();
@@ -330,7 +425,10 @@ private:
 // batch runs with its own tenant's keys.  Execution is B200Public's (replicas, slots, fused chunks, the zero-digit redo).
 class B200Server {
 public:
-  B200Server(const CKKSParameters &params, int capacity, int device) {
+  // maxTenants < 0 or == capacity: tenant id = bank region, filled when the keys are added.  maxTenants > capacity: paging (KeyPager)
+  B200Server(const CKKSParameters &params, int capacity, int device, int maxTenants = -1) {
+    if (maxTenants >= 0 && maxTenants < capacity)
+      throw std::invalid_argument("max_tenants (" + std::to_string(maxTenants) + ") is below the number of device slots (capacity " + std::to_string(capacity) + ")");
     std::vector<int> bits(params.primeBits.begin(), params.primeBits.end());
     auto s = std::make_shared<Shared>();
     s->dev = std::make_shared<Device>(params.polyModulusDegree, hmod::createCoeffModulus(params.polyModulusDegree, bits), device);
@@ -342,6 +440,7 @@ public:
       elts.insert(elt);
     }
     s->bank = std::make_unique<KeyBank>(s->dev, elts, capacity);
+    if (maxTenants > capacity) s->pager = std::make_unique<KeyPager>(s->dev, *s->bank, maxTenants);
     pub_ = std::make_unique<B200Public>(s);
   }
   // host images [k-1][2][k][N] (shapes checked by the caller); every element of the rotation set must be present
@@ -349,13 +448,46 @@ public:
     for (u64 e : bank().elements())
       if (!galois.count(e)) throw std::invalid_argument("Galois key for element " + std::to_string(e) + " of the server's rotation set is missing");
     std::lock_guard<std::mutex> guard(shared()->execMutex);
-    return shared()->bank->add(relin, galois);
+    return shared()->pager ? shared()->pager->add(relin, galois) : shared()->bank->add(relin, galois);
   }
   void removeKeys(int t) {
     std::lock_guard<std::mutex> guard(shared()->execMutex);
-    shared()->bank->requireOccupied(t);
+    shared()->requireTenant(t);
     if (pub_->tenantInFlightLocked(t)) throw std::runtime_error("tenant " + std::to_string(t) + " is used by a batch that has not been collected");
-    shared()->bank->remove(t);
+    if (shared()->pager) shared()->pager->remove(t);
+    else shared()->bank->remove(t);
+  }
+  // device-resident hooks: stage a plan replica's inputs for (tenant, valuation) requests, and run it.  With paging, run resolves the
+  // staged tenants again (a tenant evicted since is filled again) and waits / records as enqueueLocked does
+  void stageInputs(Program &prog, const std::vector<std::pair<int, const B200Valuation *>> &rq, void *stream, int replica) {
+    std::vector<int> tenants;
+    for (auto &r : rq) tenants.push_back(r.first);
+    std::lock_guard<std::mutex> guard(shared()->execMutex);
+    for (int t : tenants) shared()->requireTenant(t);
+    Executor &ex = pub_->executorFor(prog, (int)rq.size(), replica);
+    staged_[&ex] = tenants;
+    setSlots(ex, shared()->slotsFor(tenants), stream);
+    for (std::size_t b = 0; b < rq.size(); b++) pub_->stageInputs(ex, prog, *rq[b].second, stream, (int)b);
+  }
+  // tenants: replaces the staged tenants of the replica (same count)
+  void runResident(Program &prog, void *stream, int batch, int replica, const std::vector<int> &tenants = {}) {
+    std::lock_guard<std::mutex> guard(shared()->execMutex);
+    Executor &ex = pub_->executorFor(prog, batch, replica);
+    if (!tenants.empty()) {
+      if ((int)tenants.size() != batch) throw std::invalid_argument("run_resident: one tenant per instance");
+      for (int t : tenants) shared()->requireTenant(t);
+      staged_[&ex] = tenants;
+    }
+    KeyPager *pager = shared()->pager.get();
+    auto it = staged_.find(&ex);
+    if (!pager && it == staged_.end()) { ex.run(stream); return; }
+    if (it == staged_.end()) throw std::runtime_error("run_resident: stage the replica's inputs first");
+    if (pager) for (int t : it->second) pager->requireRegistered(t);
+    const std::vector<int> slots = shared()->slotsFor(it->second);
+    setSlots(ex, slots, stream);
+    if (pager) pager->beforeRun(stream, slots.data(), batch);
+    ex.run(stream);
+    if (pager) pager->afterRun(stream, slots.data(), batch);
   }
   std::shared_ptr<PendingBatch> submit(Program &program, const std::vector<std::pair<int, const B200Valuation *>> &requests, int slot = 0) {
     std::vector<const B200Valuation *> in;
@@ -372,7 +504,14 @@ public:
   std::shared_ptr<Shared> shared() const { return pub_->shared(); }
 
 private:
+  // the executor's page-locked tenant table is read by its previous run's stream-ordered upload: rewritten only after that run
+  void setSlots(Executor &ex, const std::vector<int> &slots, void *stream) {
+    if (ex.tenantsAre(slots.data(), (int)slots.size())) return;
+    shared()->dev->sync(stream);
+    ex.setTenants(slots.data(), (int)slots.size());
+  }
   std::unique_ptr<B200Public> pub_;
+  std::map<const Executor *, std::vector<int>> staged_;   // device-resident hooks: the tenants staged on a plan replica
 };
 
 class B200Secret {

@@ -32,8 +32,9 @@ struct KeyBankGuard {
 
 // Evaluation keys of up to `capacity` tenants (one client's key set each) in one device allocation.  Every tenant's region has
 // the same layout -- the relinearization key, one Galois key per element of the rotation set, then the hoist constants cadd of
-// every (element, ell) with ell = 1 .. k-1 (evab_rotate_hoist_const, filled when the tenant is added) -- so tenant t's copy of
-// any of them is at tenant 0's pointer + t * stride() words.  Plans take tenant 0's pointers and select per instance at run time.
+// every (element, ell) with ell = 1 .. k-1 (one evab_rotate_hoist_const_levels call, when the region is filled) -- so region t's
+// copy of any of them is at region 0's pointer + t * stride() words.  Plans take region 0's pointers and select per instance at
+// run time.  Without paging a tenant id is its region; with paging (KeyPager) the regions are slots that tenants are paged into.
 class KeyBank {
 public:
   KeyBank(std::shared_ptr<Device> dev, const std::set<u64> &elts, int capacity) : dev_(std::move(dev)), elts_(elts.begin(), elts.end()) {
@@ -45,6 +46,7 @@ public:
     stride_ = keyWords_ * (1 + elts_.size()) + constWords_ * elts_.size();
     for (u64 e : elts_) check(evab_galois_prepare(dev_->ctx(), e));
     bank_ = DBuf(dev_, stride_ * (std::size_t)capacity);
+    if (!elts_.empty()) tmp_ = DBuf(dev_, evab_rotate_hoist_const_levels_work_bytes(dev_->ctx(), (int)elts_.size()) / 8);
     used_.assign(capacity, 0);
     dev_->sync();
   }
@@ -74,20 +76,29 @@ public:
     const auto it = std::find(used_.begin(), used_.end(), 0);
     if (it == used_.end()) throw std::runtime_error("the key bank is full (" + std::to_string(capacity()) + " tenants): remove a tenant first");
     const int t = (int)(it - used_.begin());
-    u64 *base = bank_.get() + (std::size_t)t * stride_;
-    dev_->upload(base, relinKey, keyWords_ * 8);
-    DBuf tmp(dev_, (std::size_t)dev_->k() * dev_->N());
-    for (u64 e : elts_) {
-      u64 *key = const_cast<u64 *>(galois(e, t));
-      dev_->upload(key, galoisKeys.at(e), keyWords_ * 8);
-      for (int ell = 1; ell < dev_->k(); ell++)
-        check(evab_rotate_hoist_const(dev_->ctx(), ell, e, key, const_cast<u64 *>(hoistConst(e, ell, t)), tmp.get(), nullptr));
-    }
+    dev_->upload(region(t), relinKey, keyWords_ * 8);
+    for (u64 e : elts_) dev_->upload(const_cast<u64 *>(galois(e, t)), galoisKeys.at(e), keyWords_ * 8);
+    computeConstants(t, nullptr);
     dev_->sync();
     used_[t] = 1;
     return t;
   }
   void remove(int t) { requireOccupied(t); used_[t] = 0; }
+  // paging (B200Server with more tenants than regions): region `slot` takes the keys of a host block laid out as a region's keys
+  // ([relinearization key][Galois key of every element], keyWords() words) and recomputes the constants; stream-ordered, no sync
+  void fill(int slot, const u64 *hostKeys, void *stream) {
+    dev_->upload(region(slot), hostKeys, keyWords() * 8, stream);
+    computeConstants(slot, stream);
+  }
+  // the hoist constants of every (element, ell) of region `slot` from its Galois keys (one evab_rotate_hoist_const_levels call:
+  // the region's Galois keys and constants are each contiguous, in element order)
+  void computeConstants(int slot, void *stream) {
+    fills_++;
+    if (elts_.empty()) return;
+    check(evab_rotate_hoist_const_levels(dev_->ctx(), (int)elts_.size(), elts_.data(), galois(elts_[0], slot), const_cast<u64 *>(hoistConst(elts_[0], 1, slot)),
+                                         tmp_.get(), stream));
+  }
+  std::uint64_t fills() const { return fills_; }
 
 private:
   std::size_t index(u64 elt) const {
@@ -95,11 +106,13 @@ private:
     if (it == elts_.end() || *it != elt) throw std::invalid_argument("Galois key not present");
     return (std::size_t)(it - elts_.begin());
   }
+  u64 *region(int t) const { return bank_.get() + (std::size_t)t * stride_; }
   std::shared_ptr<Device> dev_;
   std::vector<u64> elts_;                 // sorted
   std::size_t keyWords_ = 0, constWords_ = 0, stride_ = 0;   // one key; the constants of one element; one tenant
   std::vector<char> used_;
-  DBuf bank_;
+  std::uint64_t fills_ = 0;               // regions filled (keys uploaded, constants computed)
+  DBuf bank_, tmp_;                       // tmp_: the indicators of computeConstants (fills are ordered on one stream at a time)
 };
 
 class Executor {
@@ -146,6 +159,7 @@ public:
     if (!bank_ || n != plan_.opt.batch) throw std::logic_error("setTenants: one tenant per instance of a bank-bound plan");
     for (int b = 0; b < n; b++) tenantHost_[b] = tenants[b];
   }
+  bool tenantsAre(const int *tenants, int n) const { return bank_ && n == plan_.opt.batch && std::equal(tenants, tenants + n, tenantHost_); }
   void run(void *stream) {
     if (rawDirty_) { evalRawAndEncodes(stream); rawDirty_ = false; }
     if (bank_) dev_->upload(tenantDev_.get(), tenantHost_, 4 * (std::size_t)plan_.opt.batch, stream);   // read by the kernels, not baked into the graph

@@ -10,6 +10,7 @@
 #include <pybind11/numpy.h>
 #include <pybind11/pybind11.h>
 #include <pybind11/stl.h>
+#include <optional>
 
 namespace py = pybind11;
 using namespace evab;
@@ -144,6 +145,30 @@ PYBIND11_MODULE(_eva_b200, m) {
     PackResult r = packArena(ps, pb);
     return py::make_tuple(r.offsets, r.waits, r.peak);
   }, py::arg("steps"), py::arg("buffers"));
+  // test hook: the key pager's residency policy alone (host/slot_cache.hpp).  Replays batches of tenant ids through a cache of
+  // `slots` slots; an entry ("remove", t) drops tenant t instead.  Returns (per entry: (slots of the instances, [(tenant, slot,
+  // evicted or -1)]), the error message, or None for a removal; fills; evictions)
+  m.def("_slot_cache", [](int slots, const std::vector<py::object> &ops) {
+    SlotCache c(slots);
+    py::list results;
+    for (auto &op : ops) {
+      if (py::isinstance<py::tuple>(op)) {   // ("remove", tenant)
+        c.drop(py::cast<int>(op.cast<py::tuple>()[1]));
+        results.append(py::none());
+        continue;
+      }
+      std::vector<SlotCache::Fill> fills;
+      try {
+        std::vector<int> s = c.assign(op.cast<std::vector<int>>(), fills);
+        py::list fl;
+        for (auto &f : fills) fl.append(py::make_tuple(f.tenant, f.slot, f.evicted));
+        results.append(py::make_tuple(s, fl));
+      } catch (const std::invalid_argument &e) {
+        results.append(py::str(e.what()));
+      }
+    }
+    return py::make_tuple(results, c.fills(), c.evictions());
+  }, py::arg("slots"), py::arg("batches"));
   // test hook: the planner alone (host/planner.hpp), without a device.  options: set_options' keywords; arena_limit 0 is no limit
   // here.  The scratch sizes are stand-ins derived from N and ell (the layout's invariants hold for any sizes)
   py::class_<ExecOptions> planOptions(m, "_PlanOptions");
@@ -413,7 +438,12 @@ PYBIND11_MODULE(_eva_b200, m) {
   py::class_<B200Server> srv(mb, "B200Server",
                              "Executes compiled programs for many clients: each client's evaluation keys are a tenant of a key bank of fixed "
                              "capacity, the plans are shared by all tenants, and every instance of a batch runs with its own tenant's keys");
-  srv.def(py::init<const CKKSParameters &, int, int>(), py::arg("params"), py::arg("capacity") = 64, py::arg("device") = 0)
+  srv.def(py::init([](const CKKSParameters &params, int capacity, int device, std::optional<int> maxTenants) {
+        return std::make_unique<B200Server>(params, capacity, device, maxTenants ? *maxTenants : -1);
+      }), py::arg("params"), py::arg("capacity") = 64, py::arg("device") = 0, py::arg("max_tenants") = py::none(),
+      "capacity: device slots (key-bank regions).  max_tenants None or == capacity: a tenant id is its slot, filled when its keys are "
+      "added.  max_tenants > capacity: up to max_tenants tenants' keys in page-locked host memory, paged into the slots (least "
+      "recently used first) as batches need them")
       .def("add_raw_keys", [](B200Server &s, const u64arr &relin, const std::map<u64, u64arr> &galois) {
         const std::size_t kk = s.shared()->dev->k(), N = s.shared()->dev->N();
         requireShape(relin, {kk - 1, 2, kk, N}, "relinearization key");
@@ -426,7 +456,7 @@ PYBIND11_MODULE(_eva_b200, m) {
         py::gil_scoped_release rel;
         return s.addKeys(relin.data(), g);
       }, py::arg("relin_key"), py::arg("galois_keys"), "copy a client's relinearization key and Galois keys (host arrays [k-1][2][k][N]) into a "
-         "free tenant slot and compute its hoist constants; returns the tenant id")
+         "free tenant slot and compute its hoist constants (with paging: into page-locked host memory, no device work); returns the tenant id")
       .def("add_keys", [](B200Server &s, B200Public &p) {
         auto src = p.shared();
         if (src->dev->N() != s.shared()->dev->N() || src->dev->primes() != s.shared()->dev->primes())
@@ -479,25 +509,34 @@ PYBIND11_MODULE(_eva_b200, m) {
       .def("bank_info", [](B200Server &s) {
         const KeyBank &b = s.bank();
         std::lock_guard<std::mutex> guard(s.shared()->execMutex);   // add / remove change the occupancy under it
+        const KeyPager *pg = s.shared()->pager.get();
         py::dict d;
-        d["capacity"] = b.capacity(); d["tenants"] = b.tenants(); d["galois_elements"] = b.elements();
+        d["capacity"] = b.capacity(); d["tenants"] = pg ? pg->tenants() : b.tenants(); d["galois_elements"] = b.elements();
         d["tenant_bytes"] = b.stride() * 8; d["key_bytes_per_tenant"] = b.keyWords() * 8; d["hoist_const_bytes_per_tenant"] = b.constWords() * 8;
         d["bank_bytes"] = b.stride() * 8 * (std::size_t)b.capacity();
+        d["device_slots"] = b.capacity();
+        d["max_tenants"] = pg ? pg->maxTenants() : b.capacity();
+        std::vector<int> resident;
+        if (pg) resident = pg->cache().resident();
+        else for (int t = 0; t < b.capacity(); t++) if (b.occupied(t)) resident.push_back(t);
+        d["resident"] = resident;
+        d["host_key_bytes"] = pg ? pg->hostBytes() : 0;
+        d["fills"] = b.fills();
+        d["evictions"] = pg ? pg->cache().evictions() : 0;
         return d;
-      })
+      }, "capacity / device_slots: key-bank regions; max_tenants: tenant ids (more than the slots: paging); resident: the tenants "
+         "holding a slot; host_key_bytes: page-locked host memory of the paged keys; fills: slots filled (keys uploaded and "
+         "constants computed); evictions: resident tenants displaced by a fill")
       .def("primes", [](B200Server &s) { return s.shared()->dev->primes(); })
       // ---- benchmark hooks (as B200Public's): device-resident execution of requests staged on a plan replica
       .def("stage_inputs", [](B200Server &s, Program &prog, const Requests &rq, std::uintptr_t stream, int replica) {
-        std::vector<int> tenants;
-        for (auto &r : rq) tenants.push_back(r.first);
-        std::lock_guard<std::mutex> guard(s.shared()->execMutex);
-        for (int t : tenants) s.bank().requireOccupied(t);
-        Executor &ex = s.pub().executorFor(prog, (int)rq.size(), replica);
-        ex.setTenants(tenants.data(), (int)tenants.size());
-        for (std::size_t b = 0; b < rq.size(); b++) s.pub().stageInputs(ex, prog, *rq[b].second, (void *)stream, (int)b);
+        s.stageInputs(prog, rq, (void *)stream, replica);
       }, py::arg("program"), py::arg("requests"), py::arg("stream"), py::arg("replica") = 0)
-      .def("run_resident", [](B200Server &s, Program &prog, std::uintptr_t stream, int batch, int replica) { s.pub().executorFor(prog, batch, replica).run((void *)stream); },
-           py::arg("program"), py::arg("stream"), py::arg("batch") = 1, py::arg("replica") = 0, py::call_guard<py::gil_scoped_release>())
+      .def("run_resident", [](B200Server &s, Program &prog, std::uintptr_t stream, int batch, int replica, const std::vector<int> &tenants) {
+        s.runResident(prog, (void *)stream, batch, replica, tenants);
+      }, py::arg("program"), py::arg("stream"), py::arg("batch") = 1, py::arg("replica") = 0, py::arg("tenants") = std::vector<int>(),
+         py::call_guard<py::gil_scoped_release>(),
+         "tenants: replace the staged tenants of the replica (with paging, missing ones are filled before the run)")
       .def("debug_value", [](B200Server &s, Program &prog, std::uint64_t index, int batch, int b) { return debugValue(s.pub(), prog, index, batch, b); },
            py::arg("program"), py::arg("index"), py::arg("batch") = 1, py::arg("instance") = 0);
   defSetOptions(srv);

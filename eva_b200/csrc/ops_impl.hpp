@@ -322,6 +322,22 @@ template <class BE> int hoist_const_impl(BE &be, const CtxView &c, int ell, cons
   H.ind = tmp; H.key = key; H.out = out; H.primes = c.primes; H.ell = ell; H.k = c.k; H.N = (int)c.N;
   return be.hoist_const(H);
 }
+// cadd_g of every level ell = 1 .. k-1 for n Galois keys [n][k-1][2][k][N] (contiguous), into out [n][ell][2][ell+1][N]: the n
+// indicators, ONE forward transform of all n k rows, one element-wise pass (hoist_levels_elem).  `tmp` holds n k N words
+inline size_t hoist_const_levels_work_elems(const CtxView &c, int n) { return (size_t)n * c.k * c.N; }
+template <class BE>
+int hoist_const_levels_impl(BE &be, const CtxView &c, int n, const u32 *const *ctabs, const u64 *keys, u64 *out, u64 *tmp) {
+  if (c.k < 2) return be.error("hoist constants need at least two primes");
+  if (n < 1) return be.error("hoist constants: n must be >= 1");
+  for (int g = 0; g < n; g++)
+    if (int rc = be.hoist_indicator(tmp + (size_t)g * c.k * c.N, ctabs[g], (int)c.N, c.k)) return rc;
+  int pidx[32];
+  for (int m = 0; m < c.k; m++) pidx[m] = m;
+  if (int rc = ntt_batch_impl(be, c, false, tmp, (size_t)n * c.k, pidx, c.k)) return rc;
+  HoistLevelsArgs H;
+  H.ind = tmp; H.key = keys; H.out = out; H.primes = c.primes; H.k = c.k; H.N = (int)c.N;
+  return be.hoist_levels(H, n);
+}
 inline size_t rotate_modup_work_elems(const CtxView &c, int ell) { return (size_t)2 * (ell + 1) * c.N + (size_t)2 * c.N; }   // acc + tmp
 template <class BE>
 int rotate_modup_prepared_impl(BE &be, const CtxView &c, int ell, u64 *out, const u64 *a, const u64 *ext, const u32 *nperm, const u64 *key, const u64 *cadd, u64 *work) {

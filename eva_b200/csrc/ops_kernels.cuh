@@ -283,6 +283,46 @@ EVAB_HD void hoist_const_elem(const HoistConstArgs &A, int mi, int j) {
 // I_g as residues: row mi, coefficient j = sign bit of the coefficient-domain gather table
 EVAB_HD void hoist_indicator_elem(u64 *out, const u32 *ctab, int N, int mi, int j) { out[(size_t)mi * N + j] = EVAB_LDG(ctab + j) & 1u; }
 
+// ---- the same constants for every level ell = 1 .. k-1 of n Galois keys in one pass.  The level-ell constant of prime m is
+// NTT_m(I_g) (.) (sum_{J < ell} (q_J mod m) key[J][c][m]) mod m, so all levels share one prefix sum over J: a thread keeps the
+// 128-bit running sum of its two coefficients (at most k - 1 <= 23 products below 2^120 each: below 2^125) and, each time J
+// reaches ell - 1, reduces it once and writes level ell's row -- only the rows that exist at that level (m < ell, or m = P).
+// Every key row is read once.  Reductions are canonical for any 128-bit input, so each row equals hoist_const_elem's.
+struct HoistLevelsArgs {
+  const u64 *ind;     // [n][k][N]  NTT_m(I_g) for every prime m = 0 .. k-1
+  const u64 *key;     // [n][k-1][2][k][N]
+  u64 *out;           // [n][ell = 1 .. k-1][2][ell+1][N]
+  const PrimeDev *primes;
+  int k, N;
+};
+// words of the constants of one key: sum_{ell=1}^{k-1} 2 (ell + 1) N
+EVAB_HD size_t hoist_levels_words(int k, size_t N) { return (size_t)((k + 1) * k - 2) * N; }
+EVAB_HD void hoist_levels_elem(const HoistLevelsArgs &A, int g, int m, int j) {
+  const int k = A.k;
+  const size_t N = A.N;
+  const PrimeDev P = A.primes[m];
+  const u64x2 ni = ld2(A.ind + ((size_t)g * k + m) * N + j);
+  const u64 *key = A.key + (size_t)g * (k - 1) * 2 * k * N + (size_t)m * N + j;
+  u64 *out = A.out + (size_t)g * hoist_levels_words(k, N) + j;
+  u64 l0x = 0, h0x = 0, l0y = 0, h0y = 0, l1x = 0, h1x = 0, l1y = 0, h1y = 0;
+  for (int J = 0; J < k - 1; J++) {
+    const u64 qj = A.primes[J].p % P.p;
+    const u64x2 k0 = ld2(key + ((size_t)J * 2 + 0) * k * N), k1 = ld2(key + ((size_t)J * 2 + 1) * k * N);
+    mac128(l0x, h0x, qj, k0.x); mac128(l0y, h0y, qj, k0.y);
+    mac128(l1x, h1x, qj, k1.x); mac128(l1y, h1y, qj, k1.y);
+    const int ell = J + 1;   // the sum now covers J < ell
+    if (m < ell || m == k - 1) {
+      const int mi = m == k - 1 ? ell : m;
+      u64x2 r0, r1;
+      r0.x = mulmod_p(reduce128(l0x, h0x, P), ni.x, P); r0.y = mulmod_p(reduce128(l0y, h0y, P), ni.y, P);
+      r1.x = mulmod_p(reduce128(l1x, h1x, P), ni.x, P); r1.y = mulmod_p(reduce128(l1y, h1y, P), ni.y, P);
+      st2(out + (size_t)mi * N, r0);
+      st2(out + ((size_t)ell + 1 + mi) * N, r1);
+    }
+    out += (size_t)2 * (ell + 1) * N;
+  }
+}
+
 // ---- rotate_wsum (exact): sums of rotations of one ciphertext weighted by scalar plaintexts (ops_impl.hpp rotate_wsum_impl).
 // A scalar weight is a constant polynomial: in the NTT domain one number w_r per residue, read at pt[r * N].  With acc_i the
 // key-switch accumulator of rotation i and tmp_i = iNTT_P(acc_i's P row) + floor(P/2), every output word is

@@ -203,6 +203,16 @@ int evab_rotate_modup_prepare(evab_ctx *ctx, int ell, uint64_t *d_that, uint64_t
 int evab_rotate_hoist_const(evab_ctx *ctx, int ell, uint64_t galois_elt, const uint64_t *d_key, uint64_t *d_cadd, uint64_t *d_tmp, void *stream);
 int evab_rotate_modup_prepared(evab_ctx *ctx, int ell, uint64_t *d_out, const uint64_t *d_a, const uint64_t *d_ext, uint64_t galois_elt,
                                const uint64_t *d_key, const uint64_t *d_cadd, void *d_work, void *stream);
+/* evab_rotate_hoist_const of EVERY level ell = 1 .. k-1 for n Galois keys in one pass: d_keys holds the n keys back to back
+ * ([n][k-1][2][k][N]; key g is for galois_elts[g], each prepared with evab_galois_prepare), d_out receives for key g the block
+ * [ell = 1 .. k-1][2][ell+1][N] at g * evab_hoist_const_levels_bytes(ctx) / 8 words -- level ell's [2][ell+1][N] equals
+ * evab_rotate_hoist_const(ell) bit for bit.  One batched forward transform of the n indicators over all k primes and one
+ * element-wise launch that reads every key row once.  d_tmp: evab_rotate_hoist_const_levels_work_bytes(ctx, n) bytes (n k N
+ * words).  Stream-ordered; does not synchronise.  k >= 2, n <= 65535. */
+size_t evab_hoist_const_levels_bytes(const evab_ctx *ctx);
+size_t evab_rotate_hoist_const_levels_work_bytes(const evab_ctx *ctx, int n);
+int evab_rotate_hoist_const_levels(evab_ctx *ctx, int n, const uint64_t *galois_elts, const uint64_t *d_keys, uint64_t *d_out, uint64_t *d_tmp,
+                                   void *stream);
 /* n <= 16 rotations of ONE ciphertext (seal::Evaluator::rotate_vector, seal_executor.h:176-189) in three kernel launches instead of
  * 3 n: d_out [n][2][ell][N], rotation i by galois_elts[i]; same bits as n calls of evab_rotate_modup_prepared.  d_ext, keys, cadds as there. */
 /* evab_rotate_modup_many and evab_lazy_rotsum read P * c0 from the diagonal of d_ext (ext[m][J] has no entry for m = q_J): call this once
