@@ -24,6 +24,7 @@ _SIGS = {
     "evab_malloc": (ci, [vp, szt, C.POINTER(vp), vp]),
     "evab_free": (ci, [vp, vp, vp]),
     "evab_upload": (ci, [vp, vp, vp, szt, vp]),
+    "evab_upload_2d": (ci, [vp, vp, szt, vp, szt, szt, szt, vp]),
     "evab_download": (ci, [vp, vp, vp, szt, vp]),
     "evab_sync": (ci, [vp, vp]),
     "evab_stream_create": (ci, [vp, C.POINTER(vp)]),
@@ -47,6 +48,7 @@ _SIGS = {
     "evab_hoist_const_levels_bytes": (szt, [vp]),
     "evab_rotate_hoist_const_levels_work_bytes": (szt, [vp, ci]),
     "evab_rotate_hoist_const_levels": (ci, [vp, ci, u64p, vp, vp, vp, vp]),
+    "evab_expand_key_uniform": (ci, [vp, ci, vp, u64p, vp, vp]),
     "evab_rotate_modup_prepared": (ci, [vp, ci, vp, vp, vp, u64, vp, vp, vp, vp]),
     "evab_memset_zero": (ci, [vp, vp, szt, vp]),
     "evab_rotate_modup_scale_c0": (ci, [vp, ci, vp, vp, vp]),

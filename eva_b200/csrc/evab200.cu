@@ -5,6 +5,7 @@
 #include "../../include/evab200.h"
 #include "host_tables.hpp"
 #include "ops_impl.hpp"
+#include "key_expand.cuh"
 #include <cuda_runtime.h>
 #include <atomic>
 #include <cstdlib>
@@ -259,6 +260,11 @@ __global__ void __launch_bounds__(256) k_hoist_const(const HoistConstArgs A) {
 // grid (coefficient tiles, prime m, key g)
 __global__ void __launch_bounds__(256) k_hoist_const_levels(const HoistLevelsArgs A) {
   for (int j = (blockIdx.x * blockDim.x + threadIdx.x) * 2; j < A.N; j += gridDim.x * blockDim.x * 2) hoist_levels_elem(A, blockIdx.z, blockIdx.y, j);
+}
+// grid (blocks of 8 coefficients, c1 row r, key g): one ChaCha20 block per thread
+__global__ void __launch_bounds__(256) k_expand_uniform(const ExpandArgs A) {
+  const u32 t = blockIdx.x * blockDim.x + threadIdx.x;
+  if (t < A.N / 8) expand_uniform_elem(A, blockIdx.z, blockIdx.y, t);
 }
 __global__ void __launch_bounds__(256) k_hoist_indicator(u64 *out, const u32 *ctab, int N) {
   for (int j = blockIdx.x * blockDim.x + threadIdx.x; j < N; j += gridDim.x * blockDim.x) hoist_indicator_elem(out, ctab, N, blockIdx.y, j);
@@ -666,6 +672,11 @@ extern "C" int evab_upload(evab_ctx *c, void *d, const void *h, size_t bytes, vo
   CUDA_OK(cudaMemcpyAsync(d, h, bytes, cudaMemcpyHostToDevice, S(stream)));
   return 0;
 }
+extern "C" int evab_upload_2d(evab_ctx *c, void *dst, size_t dpitch, const void *src, size_t spitch, size_t width, size_t height, void *stream) {
+  CUDA_OK(cudaSetDevice(c->device));
+  CUDA_OK(cudaMemcpy2DAsync(dst, dpitch, src, spitch, width, height, cudaMemcpyHostToDevice, S(stream)));
+  return 0;
+}
 extern "C" int evab_download(evab_ctx *c, void *h, const void *d, size_t bytes, void *stream) {
   CUDA_OK(cudaSetDevice(c->device));
   CUDA_OK(cudaMemcpyAsync(h, d, bytes, cudaMemcpyDeviceToHost, S(stream)));
@@ -949,4 +960,20 @@ extern "C" int evab_rotate(evab_ctx *c, int ell, uint64_t *o, const uint64_t *a,
     perm = it->second;
   }
   BE_BEGIN return rotate_impl(be, c->v, ell, o, a, perm, key, (u64 *)work);
+}
+extern "C" int evab_expand_key_uniform(evab_ctx *c, int n, const uint8_t *seeds, const uint64_t *moduli, uint64_t *keys, void *stream) {
+  if (n < 1 || n > 65535) return fail("evab_expand_key_uniform: n must be in [1, 65535]");
+  if (c->v.k < 2 || c->v.k > KX_MAXK) return fail("evab_expand_key_uniform: 2 <= k <= 64 primes");
+  if (!moduli) return fail("evab_expand_key_uniform: no moduli");
+  ExpandArgs A{};
+  A.seeds = reinterpret_cast<const uint32_t *>(seeds); A.keys = keys; A.N = (uint32_t)c->v.N; A.k = (uint32_t)c->v.k;
+  for (int m = 0; m < c->v.k; m++) {
+    if (moduli[m] < 2) return fail("evab_expand_key_uniform: every modulus must be >= 2");
+    A.q[m] = moduli[m]; A.lim[m] = kx_limit(moduli[m]);
+  }
+  CUDA_OK(cudaSetDevice(c->device));
+  c->launches.fetch_add(1, std::memory_order_relaxed);
+  k_expand_uniform<<<dim3((A.N / 8 + 255) / 256, (A.k - 1) * A.k, n), 256, 0, S(stream)>>>(A);
+  CUDA_OK(cudaGetLastError());
+  return 0;
 }

@@ -51,50 +51,53 @@ public:
 };
 
 // Paging of evaluation keys (B200Server with more tenants than key-bank regions): every registered tenant's keys live in a
-// page-locked host block, and the bank's regions are device slots holding the keys of the tenants used recently (SlotCache).
+// page-locked host block (in full, or compressed: c0 rows and seeds, expanded on the device at every fill), and the bank's regions are device slots holding the keys of the tenants used recently (SlotCache).
 // A batch's missing tenants are filled on the pager's own stream: a fill waits for the runs that may still read its slot (one
 // reader event per slot and replica stream), uploads the keys, recomputes the slot's hoist constants and records the slot's fill
 // event, which every run that reads the slot waits for.  The host never blocks on the way.
 class KeyPager {
 public:
   KeyPager(std::shared_ptr<Device> dev, KeyBank &bank, int maxTenants)
-      : dev_(std::move(dev)), bank_(bank), cache_(bank.capacity()), host_(maxTenants, nullptr), fillEv_(bank.capacity(), nullptr), readers_(bank.capacity()) {
+      : dev_(std::move(dev)), bank_(bank), cache_(bank.capacity()), host_(maxTenants), fillEv_(bank.capacity(), nullptr), readers_(bank.capacity()) {
     check(evab_stream_create(dev_->ctx(), &stream_));
   }
   ~KeyPager() {
     evab_ctx *c = dev_->ctx();
     evab_sync(c, stream_);   // fills still reading the host blocks
-    for (u64 *h : host_) if (h) evab_host_free(h);
+    for (Block &h : host_) if (h.p) evab_host_free(h.p);
     for (void *e : fillEv_) if (e) evab_event_destroy(c, e);
     for (auto &m : readers_) for (auto &r : m) evab_event_destroy(c, r.second);
     evab_stream_destroy(c, stream_);
   }
   KeyPager(const KeyPager &) = delete;
   int maxTenants() const { return (int)host_.size(); }
-  int tenants() const { return (int)std::count_if(host_.begin(), host_.end(), [](u64 *h) { return h != nullptr; }); }
-  bool registered(int t) const { return t >= 0 && t < maxTenants() && host_[t]; }
+  int tenants() const { return (int)std::count_if(host_.begin(), host_.end(), [](const Block &h) { return h.p != nullptr; }); }
+  int compressedTenants() const { return (int)std::count_if(host_.begin(), host_.end(), [](const Block &h) { return h.p && h.compressed; }); }
+  bool registered(int t) const { return t >= 0 && t < maxTenants() && host_[t].p; }
   void requireRegistered(int t) const {
     if (!registered(t)) throw std::invalid_argument("tenant " + std::to_string(t) + " has no keys on this server");
   }
   // host images [k-1][2][k][N] of the relinearization key and of every element's Galois key (checked by the caller) into a new
   // page-locked block; no device work.  Returns the tenant id
   int add(const u64 *relinKey, const std::map<u64, const u64 *> &galoisKeys) {
-    const auto it = std::find(host_.begin(), host_.end(), nullptr);
-    if (it == host_.end()) throw std::runtime_error("the host key store is full (" + std::to_string(maxTenants()) + " tenants): remove a tenant first");
-    const std::size_t kw = bank_.keyWords() / (1 + bank_.elements().size());
-    u64 *h = nullptr;
-    check(evab_host_alloc(bank_.keyWords() * 8, (void **)&h));
-    std::memcpy(h, relinKey, kw * 8);
-    for (std::size_t i = 0; i < bank_.elements().size(); i++) std::memcpy(h + kw * (1 + i), galoisKeys.at(bank_.elements()[i]), kw * 8);
-    *it = h;
-    return (int)(it - host_.begin());
+    Block &b = freeBlock(bank_.keyWords(), false);
+    const std::size_t kw = bank_.keyWords() / bank_.keys();
+    std::memcpy(b.p, relinKey, kw * 8);
+    for (std::size_t i = 0; i < bank_.elements().size(); i++) std::memcpy(b.p + kw * (1 + i), galoisKeys.at(bank_.elements()[i]), kw * 8);
+    return (int)(&b - host_.data());
+  }
+  // a compressed tenant: c0 rows and seeds (KeyBank::packCompressed), half the bytes of a full one
+  int addCompressed(const u64 *relinC0, const KeySeed &relinSeed, const std::map<u64, std::pair<const u64 *, KeySeed>> &galois) {
+    Block &b = freeBlock(bank_.compressedWords(), true);
+    bank_.packCompressed(b.p, relinC0, relinSeed, galois);
+    return (int)(&b - host_.data());
   }
   void remove(int t) {
     requireRegistered(t);
     cache_.drop(t);
     check(evab_sync(dev_->ctx(), stream_));   // a fill may still be reading the block
-    evab_host_free(host_[t]);
-    host_[t] = nullptr;
+    evab_host_free(host_[t].p);
+    host_[t] = Block();
   }
   // the slot of every instance of a batch; the missing tenants' fills are enqueued on the pager's stream
   std::vector<int> resolve(const std::vector<int> &tenants) {
@@ -103,7 +106,9 @@ public:
     std::vector<int> slots = cache_.assign(tenants, fills);
     for (auto &f : fills) {
       for (auto &r : readers_[f.slot]) check(evab_stream_wait_event(c, stream_, r.second));
-      bank_.fill(f.slot, host_[f.tenant], stream_);
+      const Block &b = host_[f.tenant];
+      if (b.compressed) bank_.fillCompressed(f.slot, b.p, stream_);
+      else bank_.fill(f.slot, b.p, stream_);
       if (!fillEv_[f.slot]) check(evab_event_create(c, &fillEv_[f.slot]));
       check(evab_event_record(c, fillEv_[f.slot], stream_));
     }
@@ -123,13 +128,29 @@ public:
     }
   }
   const SlotCache &cache() const { return cache_; }
-  std::size_t hostBytes() const { return (std::size_t)tenants() * bank_.keyWords() * 8; }
+  std::size_t hostBytes() const {
+    std::size_t w = 0;
+    for (const Block &b : host_) w += b.words;
+    return w * 8;
+  }
 
 private:
+  struct Block {
+    u64 *p = nullptr;          // page-locked; null: free id
+    std::size_t words = 0;     // KeyBank::keyWords() (full) or compressedWords()
+    bool compressed = false;
+  };
+  Block &freeBlock(std::size_t words, bool compressed) {
+    const auto it = std::find_if(host_.begin(), host_.end(), [](const Block &h) { return h.p == nullptr; });
+    if (it == host_.end()) throw std::runtime_error("the host key store is full (" + std::to_string(maxTenants()) + " tenants): remove a tenant first");
+    check(evab_host_alloc(words * 8, (void **)&it->p));
+    it->words = words; it->compressed = compressed;
+    return *it;
+  }
   std::shared_ptr<Device> dev_;
   KeyBank &bank_;
   SlotCache cache_;
-  std::vector<u64 *> host_;                         // tenant -> page-locked keys (keyWords() words), null: free id
+  std::vector<Block> host_;                         // tenant -> page-locked keys
   std::vector<void *> fillEv_;                      // slot -> event of its last fill
   std::vector<std::map<void *, void *>> readers_;   // slot -> (replica stream -> event after its last run that read the slot)
   void *stream_ = nullptr;                          // fills
@@ -449,6 +470,16 @@ public:
       if (!galois.count(e)) throw std::invalid_argument("Galois key for element " + std::to_string(e) + " of the server's rotation set is missing");
     std::lock_guard<std::mutex> guard(shared()->execMutex);
     return shared()->pager ? shared()->pager->add(relin, galois) : shared()->bank->add(relin, galois);
+  }
+  // compressed keys: host c0 rows [k-1][k][N] and 32-byte seeds (shapes checked by the caller); the c1 rows are expanded on the device
+  int addCompressedKeys(const u64 *relinC0, const KeySeed &relinSeed, const std::map<u64, std::pair<const u64 *, KeySeed>> &galois) {
+    for (u64 e : bank().elements())
+      if (!galois.count(e)) throw std::invalid_argument("Galois key for element " + std::to_string(e) + " of the server's rotation set is missing");
+    std::lock_guard<std::mutex> guard(shared()->execMutex);
+    if (shared()->pager) return shared()->pager->addCompressed(relinC0, relinSeed, galois);
+    std::vector<u64> image(bank().compressedWords());
+    bank().packCompressed(image.data(), relinC0, relinSeed, galois);
+    return shared()->bank->addCompressed(image.data());
   }
   void removeKeys(int t) {
     std::lock_guard<std::mutex> guard(shared()->execMutex);

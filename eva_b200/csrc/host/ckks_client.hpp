@@ -7,7 +7,9 @@
 // through the C-ABI, and so do the encoder's and the decoder's FP64 transforms; only the sampling is host code.
 #pragma once
 #include "runtime.hpp"
+#include <array>
 #include <cmath>
+#include <optional>
 #include <random>
 #include "csprng.hpp"
 
@@ -212,12 +214,35 @@ private:
   mutable DBuf zero_;
 };
 
+// the 32-byte seed from which a key-switch key's c1 rows are expanded (key_expand.cuh)
+using KeySeed = std::array<std::uint8_t, 32>;
+
+// c1 rows of the keys at d_keys [n][k-1][2][k][N] from the seeds at d_seeds [n][32] (device), modulo the context's primes
+inline void expandKeys(Device &dev, int n, const u64 *d_seeds, u64 *d_keys, void *stream) {
+  check(evab_expand_key_uniform(dev.ctx(), n, reinterpret_cast<const std::uint8_t *>(d_seeds), dev.primes().data(), d_keys, stream));
+}
+
+// a full key-switch key on the device from its compressed form: host c0 rows [k-1][k][N] and the seed
+inline DBuf expandCompressedKey(const std::shared_ptr<Device> &dev, const u64 *c0, const KeySeed &seed) {
+  const std::size_t kN = (std::size_t)dev->k() * dev->N();
+  DBuf key(dev, (std::size_t)(dev->k() - 1) * 2 * kN), d_seed(dev, 4);
+  check(evab_upload_2d(dev->ctx(), key.get(), 2 * kN * 8, c0, kN * 8, kN * 8, (std::size_t)dev->k() - 1, nullptr));
+  dev->upload(d_seed.get(), seed.data(), 32);
+  expandKeys(*dev, 1, d_seed.get(), key.get(), nullptr);
+  dev->sync();
+  return key;
+}
+
 // Secret / public / evaluation keys resident on the device.
 struct KeySet {
   DBuf sk;                       // [k][N]
   DBuf pk;                       // [2][k][N]
   DBuf relin;                    // [k-1][2][k][N]
   std::map<u64, DBuf> galois;    // galois element -> [k-1][2][k][N]
+  // seeds of the evaluation keys whose c1 rows are expanded from one (keys from generate_keys, or loaded compressed); keys
+  // supplied in full have none
+  std::optional<KeySeed> relinSeed;
+  std::map<u64, KeySeed> galoisSeeds;
 };
 
 class CkksClient {
@@ -235,7 +260,9 @@ public:
     encZeroSym(K, K.pk.get(), K.pk.get() + (std::size_t)k_ * N_);
     DBuf s2(dev_, (std::size_t)k_ * N_);
     check(evab_mul_plain(dev_->ctx(), k_, s2.get(), K.sk.get(), 1, K.sk.get(), nullptr));
-    K.relin = makeKswitchKey(K, s2.get());
+    // every evaluation key: a fresh seed from the stream (its c1 rows are expanded on the device), then its digits' errors
+    K.relinSeed = drawSeed();
+    K.relin = makeKswitchKey(K, s2.get(), *K.relinSeed);
     for (int step : rotationSteps) {
       const u64 elt = evab_galois_elt_from_step(N_, step);
       if (!elt) throw std::invalid_argument("step count too large");
@@ -244,7 +271,9 @@ public:
       // rotated secret key: one "polynomial" of k residues through the rotate-free permutation path
       DBuf rot(dev_, (std::size_t)k_ * N_);
       permute(rot.get(), K.sk.get(), elt);
-      K.galois.emplace(elt, makeKswitchKey(K, rot.get()));
+      const KeySeed seed = drawSeed();
+      K.galoisSeeds[elt] = seed;
+      K.galois.emplace(elt, makeKswitchKey(K, rot.get(), seed));
     }
     dev_->sync();
   }
@@ -322,25 +351,39 @@ private:
     dev_->sync();
     return d;
   }
+  KeySeed drawSeed() {
+    KeySeed s;
+    for (int i = 0; i < 4; i++) {
+      const u64 v = rng_();
+      for (int b = 0; b < 8; b++) s[8 * i + b] = (std::uint8_t)(v >> (8 * b));
+    }
+    return s;
+  }
   // (c0, c1) = (-(a s + e), a) at key level, NTT form
   void encZeroSym(const KeySet &K, u64 *c0, u64 *c1) {
     DBuf a = uniformDevice();
-    DBuf e = smallToDeviceNtt(sampleCbd(), k_);
     check(evab_add_plain(dev_->ctx(), k_, c1, a.get(), 1, enc_.zeroPlain(k_), nullptr));
-    check(evab_mul_plain(dev_->ctx(), k_, c0, a.get(), 1, K.sk.get(), nullptr));
+    maskWith(K, c1, c0);
+  }
+  // c0 = -(a s + e) for the uniform a at d_a, with a fresh error e
+  void maskWith(const KeySet &K, const u64 *d_a, u64 *c0) {
+    DBuf e = smallToDeviceNtt(sampleCbd(), k_);
+    check(evab_mul_plain(dev_->ctx(), k_, c0, d_a, 1, K.sk.get(), nullptr));
     check(evab_add_plain(dev_->ctx(), k_, c0, c0, 1, e.get(), nullptr));
     check(evab_negate(dev_->ctx(), k_, c0, c0, 1, nullptr));
     dev_->sync();
   }
-  // key[J] = encZeroSym with P * newKey added on residue J of component 0
-  DBuf makeKswitchKey(const KeySet &K, const u64 *d_newKey) {
+  // key[J] = (-(a_J s + e_J) + P * newKey on residue J, a_J), the a_J expanded from `seed` on the device
+  DBuf makeKswitchKey(const KeySet &K, const u64 *d_newKey, const KeySeed &seed) {
     const auto &P = dev_->primes();
-    DBuf key(dev_, (std::size_t)(k_ - 1) * 2 * k_ * N_);
+    DBuf key(dev_, (std::size_t)(k_ - 1) * 2 * k_ * N_), d_seed(dev_, 4);
+    dev_->upload(d_seed.get(), seed.data(), 32);
+    expandKeys(*dev_, 1, d_seed.get(), key.get(), nullptr);
     DBuf t(dev_, (std::size_t)k_ * N_), f(dev_, (std::size_t)k_ * N_);
     std::vector<u64> fh((std::size_t)k_ * N_);
     for (int J = 0; J < k_ - 1; J++) {
       u64 *c0 = key.get() + ((std::size_t)J * 2 + 0) * k_ * N_, *c1 = key.get() + ((std::size_t)J * 2 + 1) * k_ * N_;
-      encZeroSym(K, c0, c1);
+      maskWith(K, c1, c0);
       std::fill(fh.begin(), fh.end(), 0);
       const u64 fac = P[k_ - 1] % P[J];
       for (u64 j = 0; j < N_; j++) fh[(std::size_t)J * N_ + j] = fac;

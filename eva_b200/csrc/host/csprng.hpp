@@ -1,5 +1,6 @@
 // csprng.hpp -- the randomness of key generation and encryption (secret key, encryption masks, error
-// polynomials, the uniform halves of the public / relinearization / Galois keys).
+// polynomials, the uniform half of the public key, and the 32-byte seeds from which the device expands the uniform halves
+// of the relinearization / Galois keys, key_expand.cuh).
 //
 // The reference samples from SEAL's Blake2/SHAKE CSPRNG seeded with 512 bits.  This backend uses the ChaCha20
 // block function (RFC 8439) as a stream generator keyed with 256 bits from the operating system (getrandom(2),
@@ -10,6 +11,7 @@
 #include <cstdio>
 #include <cstring>
 #include <stdexcept>
+#include "../key_expand.cuh"
 #if defined(__linux__)
 #include <sys/random.h>
 #endif
@@ -33,10 +35,7 @@ public:
       }
       deterministic_ = true;
     }
-    static const std::uint32_t sigma[4] = {0x61707865u, 0x3320646eu, 0x79622d32u, 0x6b206574u};   // "expand 32-byte k"
-    std::memcpy(state_, sigma, 16);
-    std::memcpy(state_ + 4, key, 32);
-    state_[12] = state_[13] = state_[14] = state_[15] = 0;   // 64-bit block counter, 64-bit nonce 0 (one stream per key)
+    std::memcpy(key_, key, 32);   // the block counter starts at 0, the nonce is 0 (one stream per key)
     pos_ = 16;
     std::memset(key, 0, sizeof(key));
   }
@@ -56,22 +55,8 @@ public:
   }
 
 private:
-  static std::uint32_t rotl(std::uint32_t x, int n) { return (x << n) | (x >> (32 - n)); }
-  static void qr(std::uint32_t *s, int a, int b, int c, int d) {
-    s[a] += s[b]; s[d] ^= s[a]; s[d] = rotl(s[d], 16);
-    s[c] += s[d]; s[b] ^= s[c]; s[b] = rotl(s[b], 12);
-    s[a] += s[b]; s[d] ^= s[a]; s[d] = rotl(s[d], 8);
-    s[c] += s[d]; s[b] ^= s[c]; s[b] = rotl(s[b], 7);
-  }
   void refill() {
-    std::uint32_t x[16];
-    std::memcpy(x, state_, 64);
-    for (int i = 0; i < 10; i++) {
-      qr(x, 0, 4, 8, 12); qr(x, 1, 5, 9, 13); qr(x, 2, 6, 10, 14); qr(x, 3, 7, 11, 15);
-      qr(x, 0, 5, 10, 15); qr(x, 1, 6, 11, 12); qr(x, 2, 7, 8, 13); qr(x, 3, 4, 9, 14);
-    }
-    for (int i = 0; i < 16; i++) block_[i] = x[i] + state_[i];
-    if (++state_[12] == 0) ++state_[13];
+    chacha20_block(key_, counter_++, 0, block_);
     pos_ = 0;
   }
   static void osEntropy(void *buf, std::size_t n) {
@@ -88,7 +73,8 @@ private:
     if (!f || std::fread(buf, 1, n, f) != n) { if (f) std::fclose(f); throw std::runtime_error("no entropy source (getrandom / /dev/urandom)"); }
     std::fclose(f);
   }
-  std::uint32_t state_[16], block_[16];
+  std::uint32_t key_[8], block_[16];
+  std::uint64_t counter_ = 0;
   int pos_;
   bool deterministic_;
 };

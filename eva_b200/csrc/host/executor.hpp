@@ -46,14 +46,19 @@ public:
     stride_ = keyWords_ * (1 + elts_.size()) + constWords_ * elts_.size();
     for (u64 e : elts_) check(evab_galois_prepare(dev_->ctx(), e));
     bank_ = DBuf(dev_, stride_ * (std::size_t)capacity);
+    seeds_ = DBuf(dev_, 4 * keys() * (std::size_t)capacity);
     if (!elts_.empty()) tmp_ = DBuf(dev_, evab_rotate_hoist_const_levels_work_bytes(dev_->ctx(), (int)elts_.size()) / 8);
     used_.assign(capacity, 0);
     dev_->sync();
   }
   int capacity() const { return (int)used_.size(); }
-  int tenants() const { return (int)std::count(used_.begin(), used_.end(), 1); }
+  int tenants() const { return (int)std::count_if(used_.begin(), used_.end(), [](char u) { return u != 0; }); }
+  int compressedTenants() const { return (int)std::count(used_.begin(), used_.end(), 2); }
   std::size_t stride() const { return stride_; }                 // words
-  std::size_t keyWords() const { return keyWords_ * (1 + elts_.size()); }
+  std::size_t keys() const { return 1 + elts_.size(); }            // the relinearization key, then a Galois key per element
+  std::size_t keyWords() const { return keyWords_ * keys(); }
+  // a compressed tenant's host image: the c0 rows [k-1][k][N] of every key (in region order), then the keys' 32-byte seeds
+  std::size_t compressedWords() const { return keyWords() / 2 + 4 * keys(); }
   std::size_t constWords() const { return constWords_ * elts_.size(); }
   const std::vector<u64> &elements() const { return elts_; }
   bool has(u64 elt) const { return std::binary_search(elts_.begin(), elts_.end(), elt); }
@@ -83,11 +88,43 @@ public:
     used_[t] = 1;
     return t;
   }
+  // the same from a compressed image (compressedWords() words, packed by packCompressed): the c0 rows are uploaded, the c1 rows
+  // expanded from the seeds on the device
+  int addCompressed(const u64 *image) {
+    const auto it = std::find(used_.begin(), used_.end(), 0);
+    if (it == used_.end()) throw std::runtime_error("the key bank is full (" + std::to_string(capacity()) + " tenants): remove a tenant first");
+    const int t = (int)(it - used_.begin());
+    fillCompressed(t, image, nullptr);
+    dev_->sync();
+    *it = 2;
+    return t;
+  }
+  // host images [k-1][k][N] of the c0 rows and the seeds of the relinearization key and every element's Galois key -> dst
+  void packCompressed(u64 *dst, const u64 *relinC0, const KeySeed &relinSeed, const std::map<u64, std::pair<const u64 *, KeySeed>> &galois) const {
+    const std::size_t w = keyWords_ / 2;
+    std::memcpy(dst, relinC0, w * 8);
+    std::memcpy(dst + keys() * w, relinSeed.data(), 32);
+    for (std::size_t i = 0; i < elts_.size(); i++) {
+      const auto &g = galois.at(elts_[i]);
+      std::memcpy(dst + (1 + i) * w, g.first, w * 8);
+      std::memcpy(dst + keys() * w + 4 * (1 + i), g.second.data(), 32);
+    }
+  }
   void remove(int t) { requireOccupied(t); used_[t] = 0; }
   // paging (B200Server with more tenants than regions): region `slot` takes the keys of a host block laid out as a region's keys
   // ([relinearization key][Galois key of every element], keyWords() words) and recomputes the constants; stream-ordered, no sync
   void fill(int slot, const u64 *hostKeys, void *stream) {
     dev_->upload(region(slot), hostKeys, keyWords() * 8, stream);
+    computeConstants(slot, stream);
+  }
+  // the same from a compressed image: one strided upload puts every c0 row in its place (the digits of all keys are (k-1) keys()
+  // rows of k N words, 2 k N words apart in the region), the seeds go to the slot's seed block, one launch expands every c1 row
+  void fillCompressed(int slot, const u64 *image, void *stream) {
+    const std::size_t kN = (std::size_t)dev_->k() * dev_->N(), rows = keys() * ((std::size_t)dev_->k() - 1);
+    check(evab_upload_2d(dev_->ctx(), region(slot), 2 * kN * 8, image, kN * 8, kN * 8, rows, stream));
+    u64 *seeds = seeds_.get() + 4 * keys() * (std::size_t)slot;
+    dev_->upload(seeds, image + rows * kN, 32 * keys(), stream);
+    expandKeys(*dev_, (int)keys(), seeds, region(slot), stream);
     computeConstants(slot, stream);
   }
   // the hoist constants of every (element, ell) of region `slot` from its Galois keys (one evab_rotate_hoist_const_levels call:
@@ -110,9 +147,9 @@ private:
   std::shared_ptr<Device> dev_;
   std::vector<u64> elts_;                 // sorted
   std::size_t keyWords_ = 0, constWords_ = 0, stride_ = 0;   // one key; the constants of one element; one tenant
-  std::vector<char> used_;
+  std::vector<char> used_;                // 0: free, 1: keys added in full, 2: added compressed
   std::uint64_t fills_ = 0;               // regions filled (keys uploaded, constants computed)
-  DBuf bank_, tmp_;                       // tmp_: the indicators of computeConstants (fills are ordered on one stream at a time)
+  DBuf bank_, tmp_, seeds_;               // seeds_: [region][keys()][32 bytes], the seeds of the region's last compressed fill                       // tmp_: the indicators of computeConstants (fills are ordered on one stream at a time)
 };
 
 class Executor {

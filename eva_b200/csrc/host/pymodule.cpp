@@ -27,6 +27,16 @@ static void requireShape(const u64arr &a, std::initializer_list<std::size_t> sha
   if (!ok) throw std::runtime_error(std::string(what) + " does not match the parameters (modulus count / degree)");
 }
 
+// a key seed from Python bytes: exactly 32 of them
+static KeySeed toSeed(const py::bytes &b, const char *what) {
+  const std::string v = b;
+  if (v.size() != 32) throw std::invalid_argument(std::string(what) + " seed must be exactly 32 bytes (got " + std::to_string(v.size()) + ")");
+  KeySeed s;
+  std::memcpy(s.data(), v.data(), 32);
+  return s;
+}
+static py::bytes fromSeed(const KeySeed &s) { return py::bytes(reinterpret_cast<const char *>(s.data()), 32); }
+
 // set_options: one argument list for B200Public and for the planner test hook (_plan), which parses its options dict through it
 static ExecOptions &optionsOf(B200Public &p) { return p.options; }
 static ExecOptions &optionsOf(B200Server &s) { return s.pub().options; }
@@ -307,6 +317,13 @@ PYBIND11_MODULE(_eva_b200, m) {
         py::dict g;
         for (auto &kv : s->keys.galois) g[py::int_(kv.first)] = down(kv.second, {k - 1, 2, k, N});
         d["galois_keys"] = g;
+        // keys whose c1 rows are expanded from seeds: the seeds too (serialization then writes the compressed form)
+        if (s->keys.relinSeed && s->keys.galoisSeeds.size() == s->keys.galois.size()) {
+          d["relin_seed"] = fromSeed(*s->keys.relinSeed);
+          py::dict gs;
+          for (auto &kv : s->keys.galoisSeeds) gs[py::int_(kv.first)] = fromSeed(kv.second);
+          d["galois_seeds"] = gs;
+        }
         return d;
       })
       .def("launch_count", [](B200Public &p) { return evab_launch_count(p.shared()->dev->ctx()); })
@@ -457,30 +474,64 @@ PYBIND11_MODULE(_eva_b200, m) {
         return s.addKeys(relin.data(), g);
       }, py::arg("relin_key"), py::arg("galois_keys"), "copy a client's relinearization key and Galois keys (host arrays [k-1][2][k][N]) into a "
          "free tenant slot and compute its hoist constants (with paging: into page-locked host memory, no device work); returns the tenant id")
+      .def("add_compressed_keys", [](B200Server &s, const u64arr &relinC0, const py::bytes &relinSeed, const std::map<u64, u64arr> &galoisC0,
+                                     const std::map<u64, py::bytes> &galoisSeeds) {
+        const std::size_t kk = s.shared()->dev->k(), N = s.shared()->dev->N();
+        requireShape(relinC0, {kk - 1, kk, N}, "compressed relinearization key");
+        const KeySeed rs = toSeed(relinSeed, "relinearization key");
+        std::map<u64, std::pair<const u64 *, KeySeed>> g;   // the elements of the rotation set (addCompressedKeys reports a missing one)
+        for (u64 e : s.bank().elements()) {
+          auto it = galoisC0.find(e);
+          if (it == galoisC0.end()) continue;
+          requireShape(it->second, {kk - 1, kk, N}, "compressed Galois key");
+          auto sd = galoisSeeds.find(e);
+          if (sd == galoisSeeds.end()) throw std::invalid_argument("no seed for the Galois key of element " + std::to_string(e));
+          g[e] = {it->second.data(), toSeed(sd->second, "Galois key")};
+        }
+        py::gil_scoped_release rel;
+        return s.addCompressedKeys(relinC0.data(), rs, g);
+      }, py::arg("relin_c0"), py::arg("relin_seed"), py::arg("galois_c0"), py::arg("galois_seeds"),
+         "add a client's keys in compressed form: the c0 rows (host arrays [k-1][k][N]) and the 32-byte seed of the relinearization key "
+         "and of every Galois key; the c1 rows are expanded on the device (with paging: the compressed form is what the host store keeps, "
+         "half the bytes of add_raw_keys).  Returns the tenant id")
       .def("add_keys", [](B200Server &s, B200Public &p) {
         auto src = p.shared();
         if (src->dev->N() != s.shared()->dev->N() || src->dev->primes() != s.shared()->dev->primes())
           throw std::invalid_argument("the context's N / primes do not match the server's");
-        const std::size_t kk = s.shared()->dev->k(), words = (kk - 1) * 2 * kk * s.shared()->dev->N();
+        const std::size_t kk = s.shared()->dev->k(), kN = kk * s.shared()->dev->N(), words = (kk - 1) * 2 * kN;
         if (!src->keys.relin || src->keys.relin.words() != words) throw std::invalid_argument("the context has no relinearization key of the server's shape");
-        std::vector<u64> relin(words);
+        // keys expanded from seeds travel compressed: only their c0 rows are read back
+        bool seeded = src->keys.relinSeed.has_value();
+        for (u64 e : s.bank().elements())
+          if (src->keys.galois.count(e) && !src->keys.galoisSeeds.count(e)) seeded = false;
+        const std::size_t hw = seeded ? words / 2 : words;
+        auto fetch = [&](const DBuf &key, std::vector<u64> &h) {
+          h.resize(hw);
+          if (!seeded) { src->dev->download(h.data(), key.get(), words * 8); return; }
+          for (std::size_t J = 0; J + 1 < kk; J++) src->dev->download(h.data() + J * kN, key.get() + J * 2 * kN, kN * 8);
+        };
+        std::vector<u64> relin;
         std::map<u64, std::vector<u64>> gal;
-        std::map<u64, const u64 *> g;
         src->dev->sync();
-        src->dev->download(relin.data(), src->keys.relin.get(), words * 8);
+        fetch(src->keys.relin, relin);
         for (u64 e : s.bank().elements()) {
           auto it = src->keys.galois.find(e);
-          if (it == src->keys.galois.end()) continue;   // addKeys reports it
+          if (it == src->keys.galois.end()) continue;   // addKeys / addCompressedKeys report it
           if (it->second.words() != words) throw std::invalid_argument("Galois key does not match the server's shape");
-          auto &h = gal[e];
-          h.resize(words);
-          src->dev->download(h.data(), it->second.get(), words * 8);
-          g[e] = h.data();
+          fetch(it->second, gal[e]);
         }
         src->dev->sync();
         py::gil_scoped_release rel;
+        if (seeded) {
+          std::map<u64, std::pair<const u64 *, KeySeed>> g;
+          for (auto &kv : gal) g[kv.first] = {kv.second.data(), src->keys.galoisSeeds.at(kv.first)};
+          return s.addCompressedKeys(relin.data(), *src->keys.relinSeed, g);
+        }
+        std::map<u64, const u64 *> g;
+        for (auto &kv : gal) g[kv.first] = kv.second.data();
         return s.addKeys(relin.data(), g);
-      }, py::arg("public_context"), "add_raw_keys with the evaluation keys of a client's B200Public (same N and primes)")
+      }, py::arg("public_context"), "add a client's B200Public (same N and primes): compressed (add_compressed_keys) when its keys were "
+         "expanded from seeds (generate_keys, or a loaded compressed context), in full (add_raw_keys) otherwise")
       .def("remove_keys", &B200Server::removeKeys, py::arg("tenant"))
       .def("execute", [](B200Server &s, Program &prog, int tenant, const B200Valuation &in) {
         return std::move(s.executeBatch(prog, {{tenant, &in}})[0]);
@@ -521,11 +572,13 @@ PYBIND11_MODULE(_eva_b200, m) {
         else for (int t = 0; t < b.capacity(); t++) if (b.occupied(t)) resident.push_back(t);
         d["resident"] = resident;
         d["host_key_bytes"] = pg ? pg->hostBytes() : 0;
+        d["compressed_tenants"] = pg ? pg->compressedTenants() : b.compressedTenants();
         d["fills"] = b.fills();
         d["evictions"] = pg ? pg->cache().evictions() : 0;
         return d;
       }, "capacity / device_slots: key-bank regions; max_tenants: tenant ids (more than the slots: paging); resident: the tenants "
-         "holding a slot; host_key_bytes: page-locked host memory of the paged keys; fills: slots filled (keys uploaded and "
+         "holding a slot; host_key_bytes: page-locked host memory of the paged keys (compressed tenants: c0 rows and seeds); "
+         "compressed_tenants: tenants added in compressed form; fills: slots filled (keys uploaded and "
          "constants computed); evictions: resident tenants displaced by a fill")
       .def("primes", [](B200Server &s) { return s.shared()->dev->primes(); })
       // ---- benchmark hooks (as B200Public's): device-resident execution of requests staged on a plan replica
@@ -563,23 +616,44 @@ PYBIND11_MODULE(_eva_b200, m) {
     return std::make_unique<B200Public>(s);
   }, py::arg("N"), py::arg("primes"), py::arg("relin_key"), py::arg("galois_keys"), py::arg("device") = 0);
   // serialization: contexts rebuilt from saved key material
-  mb.def("public_from_raw", [](std::uint64_t N, const std::vector<u64> &primes, py::object pk, py::object relin, const std::map<u64, u64arr> &galois, int device) {
+  // relin_seed / galois_seeds: the matching keys are compressed -- c0 rows [k-1][k][N] -- and their c1 rows are expanded on the device
+  mb.def("public_from_raw", [](std::uint64_t N, const std::vector<u64> &primes, py::object pk, py::object relin, const std::map<u64, u64arr> &galois, int device,
+                               py::object relinSeed, const std::map<u64, py::bytes> &galoisSeeds) {
     auto s = std::make_shared<Shared>();
     s->dev = std::make_shared<Device>(N, primes, device);
     s->client = std::make_unique<CkksClient>(s->dev, 0);   // OS entropy (csprng.hpp)
     auto up = [&](DBuf &dst, const u64arr &a) { dst = DBuf(s->dev, a.size()); s->dev->upload(dst.get(), a.data(), a.size() * 8); s->dev->sync(); };
     const std::size_t kk = primes.size();
+    for (auto &g : galoisSeeds) if (!galois.count(g.first)) throw std::invalid_argument("a Galois seed without its key");
     if (!pk.is_none()) { requireShape(py::cast<u64arr>(pk), {2, kk, (std::size_t)N}, "public key"); up(s->keys.pk, py::cast<u64arr>(pk)); }
-    if (!relin.is_none()) { requireShape(py::cast<u64arr>(relin), {kk - 1, 2, kk, (std::size_t)N}, "relinearization key"); up(s->keys.relin, py::cast<u64arr>(relin)); }
-    for (auto &g : galois) requireShape(g.second, {kk - 1, 2, kk, (std::size_t)N}, "Galois key");
+    if (!relin.is_none()) {
+      const u64arr r = py::cast<u64arr>(relin);
+      if (relinSeed.is_none()) { requireShape(r, {kk - 1, 2, kk, (std::size_t)N}, "relinearization key"); up(s->keys.relin, r); }
+      else {
+        requireShape(r, {kk - 1, kk, (std::size_t)N}, "compressed relinearization key");
+        s->keys.relinSeed = toSeed(py::cast<py::bytes>(relinSeed), "relinearization key");
+        s->keys.relin = expandCompressedKey(s->dev, r.data(), *s->keys.relinSeed);
+      }
+    }
+    for (auto &g : galois) {
+      if (galoisSeeds.count(g.first)) requireShape(g.second, {kk - 1, kk, (std::size_t)N}, "compressed Galois key");
+      else requireShape(g.second, {kk - 1, 2, kk, (std::size_t)N}, "Galois key");
+    }
     for (auto &g : galois) {
       check(evab_galois_prepare(s->dev->ctx(), g.first));
       DBuf d;
-      up(d, g.second);
+      if (auto sd = galoisSeeds.find(g.first); sd != galoisSeeds.end()) {
+        const KeySeed seed = toSeed(sd->second, "Galois key");
+        s->keys.galoisSeeds[g.first] = seed;
+        d = expandCompressedKey(s->dev, g.second.data(), seed);
+      } else {
+        up(d, g.second);
+      }
       s->keys.galois.emplace(g.first, std::move(d));
     }
     return std::make_unique<B200Public>(s);
-  }, py::arg("N"), py::arg("primes"), py::arg("public_key"), py::arg("relin_key"), py::arg("galois_keys"), py::arg("device") = 0);
+  }, py::arg("N"), py::arg("primes"), py::arg("public_key"), py::arg("relin_key"), py::arg("galois_keys"), py::arg("device") = 0,
+     py::arg("relin_seed") = py::none(), py::arg("galois_seeds") = std::map<u64, py::bytes>());
   mb.def("secret_from_raw", [](std::uint64_t N, const std::vector<u64> &primes, const u64arr &sk, int device) {
     auto s = std::make_shared<Shared>();
     s->dev = std::make_shared<Device>(N, primes, device);

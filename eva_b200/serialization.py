@@ -139,6 +139,9 @@ _ATTRS = {1: ("RescaleDivisorAttribute", "uint32"), 2: ("RotationAttribute", "in
           7: ("EncodeAtLevelAttribute", "uint32")}
 _KEY_OF = {v[0]: k for k, v in _ATTRS.items()}
 (CIPHERTEXT, PLAINTEXT, SECRET_KEY, PUBLIC_KEY, GALOIS_KEYS, RELIN_KEYS, ENCRYPTION_PARAMETERS) = range(1, 8)
+# payload kinds (EVAB header only) of seed-compressed keys, under the RELIN_KEYS / GALOIS_KEYS objects: the c0 rows [k-1][k][N] of
+# every key, and in the header's extra words its 32-byte seed as 4 little-endian u64 words (Galois: the elements, then the seeds)
+COMPRESSED_RELIN_KEYS, COMPRESSED_GALOIS_KEYS = 16, 17
 
 
 # ------------------------------------------------------------------ Program / parameters / signature
@@ -284,18 +287,39 @@ def _params_from(msg_obj):
     return int(extra[0]), [int(p) for p in primes]
 
 
+def _seed_words(seed):
+    return list(struct.unpack("<4Q", seed))
+
+
+def _seed_bytes(words):
+    return struct.pack("<4Q", *words)
+
+
+def _kind(data):
+    return struct.unpack_from("<4sB", data, 0)[1]
+
+
 def public_to_msg(ctx):
     d = ctx._export()
     msg = _cls("SEALPublic")()
     _params_obj(msg.encryption_parameters, d["N"], d["primes"])
+    compressed = "relin_seed" in d        # keys expanded from seeds are written as c0 rows + seeds: half the bytes
     if "public_key" in d:
         msg.public_key.seal_type, msg.public_key.data = PUBLIC_KEY, _pack(PUBLIC_KEY, d["public_key"])
     if "relin_key" in d:
-        msg.relin_keys.seal_type, msg.relin_keys.data = RELIN_KEYS, _pack(RELIN_KEYS, d["relin_key"])
+        msg.relin_keys.seal_type = RELIN_KEYS
+        if compressed:
+            msg.relin_keys.data = _pack(COMPRESSED_RELIN_KEYS, d["relin_key"][:, 0], extra=_seed_words(d["relin_seed"]))
+        else:
+            msg.relin_keys.data = _pack(RELIN_KEYS, d["relin_key"])
     elts = sorted(d["galois_keys"])
     if elts:
         msg.galois_keys.seal_type = GALOIS_KEYS
-        msg.galois_keys.data = _pack(GALOIS_KEYS, np.stack([d["galois_keys"][e] for e in elts]), extra=elts)
+        if compressed:
+            seeds = [w for e in elts for w in _seed_words(d["galois_seeds"][e])]
+            msg.galois_keys.data = _pack(COMPRESSED_GALOIS_KEYS, np.stack([d["galois_keys"][e][:, 0] for e in elts]), extra=elts + seeds)
+        else:
+            msg.galois_keys.data = _pack(GALOIS_KEYS, np.stack([d["galois_keys"][e] for e in elts]), extra=elts)
     return msg
 
 
@@ -303,12 +327,28 @@ def public_from_msg(msg, device=0):
     from . import b200
     N, primes = _params_from(msg.encryption_parameters)
     pk = _unpack(msg.public_key.data, PUBLIC_KEY)[0] if msg.public_key.data else None
-    rk = _unpack(msg.relin_keys.data, RELIN_KEYS)[0] if msg.relin_keys.data else None
-    gal = {}
+    rk, rseed = None, None
+    if msg.relin_keys.data:
+        if _kind(msg.relin_keys.data) == COMPRESSED_RELIN_KEYS:
+            rk, _, words = _unpack(msg.relin_keys.data, COMPRESSED_RELIN_KEYS)
+            if len(words) != 4:
+                raise RuntimeError("compressed relinearization key: the seed must be 32 bytes")
+            rseed = _seed_bytes(words)
+        else:
+            rk = _unpack(msg.relin_keys.data, RELIN_KEYS)[0]
+    gal, gseeds = {}, {}
     if msg.galois_keys.data:
-        arr, _, elts = _unpack(msg.galois_keys.data, GALOIS_KEYS)
+        if _kind(msg.galois_keys.data) == COMPRESSED_GALOIS_KEYS:
+            arr, _, extra = _unpack(msg.galois_keys.data, COMPRESSED_GALOIS_KEYS)
+            n = arr.shape[0]
+            if len(extra) != 5 * n:
+                raise RuntimeError("compressed Galois keys: one element and one 32-byte seed per key")
+            elts = extra[:n]
+            gseeds = {int(e): _seed_bytes(extra[n + 4 * i:n + 4 * i + 4]) for i, e in enumerate(elts)}
+        else:
+            arr, _, elts = _unpack(msg.galois_keys.data, GALOIS_KEYS)
         gal = {int(e): np.ascontiguousarray(arr[i]) for i, e in enumerate(elts)}
-    return b200.public_from_raw(N, primes, pk, rk, gal, device)
+    return b200.public_from_raw(N, primes, pk, rk, gal, device, relin_seed=rseed, galois_seeds=gseeds)
 
 
 def secret_to_msg(ctx):

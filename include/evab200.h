@@ -51,6 +51,9 @@ int evab_mem_info(evab_ctx *ctx, size_t *free_bytes, size_t *total_bytes);
 int evab_malloc(evab_ctx *ctx, size_t bytes, void **d_ptr, void *stream);
 int evab_free(evab_ctx *ctx, void *d_ptr, void *stream);
 int evab_upload(evab_ctx *ctx, void *d_dst, const void *h_src, size_t bytes, void *stream);
+/* `height` rows of `width` bytes, row i from h_src + i * spitch to d_dst + i * dpitch (one strided copy: the c0 rows of
+ * compressed keys into their places in the key layout) */
+int evab_upload_2d(evab_ctx *ctx, void *d_dst, size_t dpitch, const void *h_src, size_t spitch, size_t width, size_t height, void *stream);
 int evab_download(evab_ctx *ctx, void *h_dst, const void *d_src, size_t bytes, void *stream);
 int evab_sync(evab_ctx *ctx, void *stream); /* blocks the calling thread */
 /* page-locked host memory for ciphertext / plaintext buffers that cross the boundary: uploads and
@@ -213,6 +216,12 @@ size_t evab_hoist_const_levels_bytes(const evab_ctx *ctx);
 size_t evab_rotate_hoist_const_levels_work_bytes(const evab_ctx *ctx, int n);
 int evab_rotate_hoist_const_levels(evab_ctx *ctx, int n, const uint64_t *galois_elts, const uint64_t *d_keys, uint64_t *d_out, uint64_t *d_tmp,
                                    void *stream);
+/* Seed-compressed key-switch keys: a key whose c1 rows (the uniform halves) are not stored but expanded from a 32-byte seed by
+ * the rule of eva_b200/csrc/key_expand.cuh (ChaCha20 blocks keyed by the seed, rejection sampling mod q; DESIGN §2).  Writes the
+ * c1 rows of n keys d_keys [n][k-1][2][k][N]: row (J, m) of key g from the seed d_seeds[g] (device, [n][32] bytes) modulo
+ * h_moduli[m] (host array of the k moduli, read during the call; the context's primes for real keys, any moduli >= 2 for
+ * tests).  The c0 rows are not touched.  One launch; stream-ordered, does not synchronise.  1 <= n <= 65535, k <= 64. */
+int evab_expand_key_uniform(evab_ctx *ctx, int n, const uint8_t *d_seeds, const uint64_t *h_moduli, uint64_t *d_keys, void *stream);
 /* n <= 16 rotations of ONE ciphertext (seal::Evaluator::rotate_vector, seal_executor.h:176-189) in three kernel launches instead of
  * 3 n: d_out [n][2][ell][N], rotation i by galois_elts[i]; same bits as n calls of evab_rotate_modup_prepared.  d_ext, keys, cadds as there. */
 /* evab_rotate_modup_many and evab_lazy_rotsum read P * c0 from the diagonal of d_ext (ext[m][J] has no entry for m = q_J): call this once

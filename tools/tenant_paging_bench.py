@@ -8,9 +8,13 @@ under these arms, alternating within each run (--runs):
   paging_miss_M    B200Server(capacity=32, max_tenants=128), 128 tenants; every step names 32 distinct tenants of which M are not
                    resident (M = 1, 8, 32): M fills per step, each waiting for the runs that read its slot
 
+Every arm also runs with compressed tenants (suffix _c: add_compressed_keys, the c0 rows and a 32-byte seed per key; a fill uploads
+the c0 rows and expands the c1 rows on the device), alternating with the full-key arms in the same run.
+
 Also measured, with CUDA events on one stream: one fill split into the key upload (page-locked host -> device) and the hoist
 constants (evab_rotate_hoist_const_levels), and one tenant's constants with the old loop of one evab_rotate_hoist_const call per
-(element, level).  Keys and ciphertexts are uniform residues (valid evaluator inputs), seeded.  The GPU name and power limit are
+(element, level); and one compressed fill split into the c0 upload (one strided evab_upload_2d, and for comparison one
+evab_upload per digit), the seed upload + expansion (evab_expand_key_uniform) and the constants.  Keys and ciphertexts are uniform residues (valid evaluator inputs), seeded.  The GPU name and power limit are
 read in the same run.
 
   python tools/tenant_paging_bench.py --workloads sobel harris --runs 2 --steps 20 --out DIR/paging.json
@@ -47,6 +51,14 @@ def keys_for(elts, primes, N, seed):
     rng = np.random.default_rng(seed)
     k = len(primes)
     return uniform(rng, primes, (k - 1, 2), k, N), {int(e): uniform(rng, primes, (k - 1, 2), k, N) for e in elts}
+
+
+def compressed(keys, seed):
+    """add_compressed_keys arguments from a key set: its c0 rows and seeded 32-byte seeds"""
+    rng = np.random.default_rng(seed)
+    rk, gk = keys
+    sd = lambda: rng.integers(0, 256, 32, dtype=np.uint8).tobytes()
+    return (np.ascontiguousarray(rk[:, 0]), sd(), {e: np.ascontiguousarray(v[:, 0]) for e, v in gk.items()}, {e: sd() for e in gk})
 
 
 class Schedule:
@@ -128,6 +140,32 @@ def fill_costs(N, primes, elts, keys, reps=10):
     torch.cuda.synchronize()
     r["levels_equal_loop"] = bool(torch.equal(out, old))
     r["fill_ms"] = r["upload_ms"] + r["constants_levels_ms"]
+    # compressed fill: the c0 rows of the n + 1 keys ((k-1) (n+1) rows of k N words, 2 k N words apart on the device)
+    kN = k * N
+    rows = (k - 1) * (n + 1)
+    c0 = torch.from_numpy(np.concatenate([keys[0][:, 0].ravel()] + [keys[1][e][:, 0].ravel() for e in elts]).view(np.int64)).pin_memory()
+    seeds = torch.from_numpy(np.random.default_rng(3).integers(0, 1 << 62, 4 * (n + 1), dtype=np.int64)).pin_memory()
+    dseeds = torch.empty_like(seeds, device="cuda")
+    hp, dp = c0.data_ptr(), dev.data_ptr()
+
+    def up2d():
+        assert lib.evab_upload_2d(h, C.c_void_p(dp), 2 * kN * 8, C.c_void_p(hp), kN * 8, kN * 8, rows, sp) == 0
+
+    def per_digit():
+        for i in range(rows):
+            assert lib.evab_upload(h, C.c_void_p(dp + 16 * kN * i), C.c_void_p(hp + 8 * kN * i), kN * 8, sp) == 0
+
+    def expand():
+        dseeds.copy_(seeds, non_blocking=True)
+        assert lib.evab_expand_key_uniform(h, n + 1, C.c_void_p(dseeds.data_ptr()), pa.ctypes.data_as(C.POINTER(C.c_uint64)), C.c_void_p(dp), sp) == 0
+
+    r.update({"c0_upload_2d_ms": timed(up2d), "c0_upload_per_digit_ms": timed(per_digit), "c0_upload_bytes": c0.numel() * 8, "c0_rows": rows,
+              "expand_ms": timed(expand), "expand_words_written": rows * kN})
+    r["compressed_fill_ms"] = r["c0_upload_2d_ms"] + r["expand_ms"] + r["constants_levels_ms"]
+
+    def fill_c():
+        up2d(); expand(); levels()
+    r["compressed_fill_together_ms"] = timed(fill_c)
     lib.evab_ctx_destroy(h)
     return r
 
@@ -193,23 +231,34 @@ def main():
         paged = b200.B200Server(params, capacity=SLOTS, max_tenants=TENANTS)
         for t in range(TENANTS):
             paged.add_raw_keys(*keysets[t % KEYSETS])
-        for s in (plain, fit, paged):
+        ckeys = [compressed(ks, 500 + i) for i, ks in enumerate(keysets)]
+        plain_c = b200.B200Server(params, capacity=SLOTS)
+        fit_c = b200.B200Server(params, capacity=SLOTS, max_tenants=TENANTS)
+        for t in range(B):
+            plain_c.add_compressed_keys(*ckeys[t % KEYSETS])
+            fit_c.add_compressed_keys(*ckeys[t % KEYSETS])
+        paged_c = b200.B200Server(params, capacity=SLOTS, max_tenants=TENANTS)
+        for t in range(TENANTS):
+            paged_c.add_compressed_keys(*ckeys[t % KEYSETS])
+        for s in (plain, fit, paged, plain_c, fit_c, paged_c):
             s.set_options(**opts)
         pub = b200.context_from_raw_keys(N, primes, *keysets[0])
         nops = pub.cipher_op_count(prog)
         del pub
         # assignments: the warm-up and every run of an arm continue one schedule, so that each step misses exactly M
-        sched = {m: Schedule(m, B) for m in args.misses}
+        sched = {(m, c): Schedule(m, B) for m in args.misses for c in ("", "_c")}
         fixed = list(range(B))
-        arms = {"no_paging": (plain, None), "paging_fit": (fit, None)}
-        arms.update({"paging_miss_%d" % m: (paged, m) for m in args.misses})
+        arms = {}
+        for c, (p0, p1, p2) in (("", (plain, fit, paged)), ("_c", (plain_c, fit_c, paged_c))):
+            arms.update({"no_paging" + c: (p0, None, c), "paging_fit" + c: (p1, None, c)})
+            arms.update({"paging_miss_%d%s" % (m, c): (p2, m, c) for m in args.misses})
 
-        def assign(m):
-            return fixed if m is None else sched[m].next()
+        def assign(m, c):
+            return fixed if m is None else sched[(m, c)].next()
 
         def e2e(name, steps):
-            srv, m = arms[name]
-            batches = [assign(m) for _ in range(steps)]
+            srv, m, c = arms[name]
+            batches = [assign(m, c) for _ in range(steps)]
             f0 = srv.bank_info()["fills"]
             dt = measure(lambda i: srv.execute_batch_async(prog, list(zip(batches[i], vals)), i & 1), srv.execute_batch_result, steps)
             return dt, (srv.bank_info()["fills"] - f0) / steps
@@ -217,14 +266,14 @@ def main():
         # device-resident: instance g of step i on replica g + 32 (i % 2) (a replica's tenant table is rewritten only after its run
         # two steps back); every replica staged once
         s0 = main_stream.cuda_stream
-        for name, (srv, m) in arms.items():
+        for name, (srv, m, c) in arms.items():
             for r in range(2 * B):
                 srv.stage_inputs(prog, [(fixed[r % B], vals[r % B])], s0, r)
         torch.cuda.synchronize()
 
         def res(name, steps):
-            srv, m = arms[name]
-            batches = [assign(m) for _ in range(steps)]
+            srv, m, c = arms[name]
+            batches = [assign(m, c) for _ in range(steps)]
             f0 = srv.bank_info()["fills"]
             dt = resident(lambda i, g, st: srv.run_resident(prog, st, 1, g + B * (i % 2), [batches[i][g]]), steps)
             return dt, (srv.bank_info()["fills"] - f0) / steps
@@ -242,7 +291,7 @@ def main():
                 dt, fps = e2e(name, args.steps)
                 e2e_rates[name].append(B * nops * args.steps / dt)
                 fills[name]["e2e"].append(fps)
-        info = paged.bank_info()
+        info, info_c = paged.bank_info(), paged_c.bank_info()
         out = {
             "cipher_ops_per_instance": nops,
             "resident_ops_per_s": {k: [round(x) for x in v] for k, v in res_rates.items()},
@@ -252,11 +301,12 @@ def main():
             "fills_per_step": fills,
             "bank": {k: info[k] for k in ("device_slots", "max_tenants", "tenant_bytes", "key_bytes_per_tenant", "hoist_const_bytes_per_tenant",
                                           "bank_bytes", "host_key_bytes", "fills", "evictions")},
+            "bank_compressed": {k: info_c[k] for k in ("host_key_bytes", "compressed_tenants", "fills", "evictions")},
             "one_fill": fill_costs(N, primes, elts, keysets[0]),
         }
         print(wl, json.dumps(out), flush=True)
         result["workloads"][wl] = out
-        del plain, fit, paged
+        del plain, fit, paged, plain_c, fit_c, paged_c
     if args.out:
         os.makedirs(os.path.dirname(os.path.abspath(args.out)), exist_ok=True)
         with open(args.out, "w") as f:
