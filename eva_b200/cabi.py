@@ -49,6 +49,7 @@ _SIGS = {
     "evab_rotate_hoist_const_levels_work_bytes": (szt, [vp, ci]),
     "evab_rotate_hoist_const_levels": (ci, [vp, ci, u64p, vp, vp, vp, vp]),
     "evab_expand_key_uniform": (ci, [vp, ci, vp, u64p, vp, vp]),
+    "evab_expand_cipher_uniform": (ci, [vp, ci, vp, vp, vp, u64p, vp]),
     "evab_rotate_modup_prepared": (ci, [vp, ci, vp, vp, vp, u64, vp, vp, vp, vp]),
     "evab_memset_zero": (ci, [vp, vp, szt, vp]),
     "evab_rotate_modup_scale_c0": (ci, [vp, ci, vp, vp, vp]),

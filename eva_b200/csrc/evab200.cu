@@ -7,8 +7,10 @@
 #include "ops_impl.hpp"
 #include "key_expand.cuh"
 #include <cuda_runtime.h>
+#include <algorithm>
 #include <atomic>
 #include <cstdlib>
+#include <cstring>
 #include <map>
 #include <mutex>
 #include <string>
@@ -265,6 +267,11 @@ __global__ void __launch_bounds__(256) k_hoist_const_levels(const HoistLevelsArg
 __global__ void __launch_bounds__(256) k_expand_uniform(const ExpandArgs A) {
   const u32 t = blockIdx.x * blockDim.x + threadIdx.x;
   if (t < A.N / 8) expand_uniform_elem(A, blockIdx.z, blockIdx.y, t);
+}
+// grid (blocks of 8 coefficients, ciphertext row m, entry i of the launch): one ChaCha20 block per thread; rows m >= ell_i return
+__global__ void __launch_bounds__(256) k_expand_cipher_uniform(const CipherExpandArgs A) {
+  const u32 t = blockIdx.x * blockDim.x + threadIdx.x;
+  if (t < A.N / 8 && blockIdx.y < A.e[blockIdx.z].ell) expand_cipher_elem(A, blockIdx.z, blockIdx.y, t);
 }
 __global__ void __launch_bounds__(256) k_hoist_indicator(u64 *out, const u32 *ctab, int N) {
   for (int j = blockIdx.x * blockDim.x + threadIdx.x; j < N; j += gridDim.x * blockDim.x) hoist_indicator_elem(out, ctab, N, blockIdx.y, j);
@@ -975,5 +982,43 @@ extern "C" int evab_expand_key_uniform(evab_ctx *c, int n, const uint8_t *seeds,
   c->launches.fetch_add(1, std::memory_order_relaxed);
   k_expand_uniform<<<dim3((A.N / 8 + 255) / 256, (A.k - 1) * A.k, n), 256, 0, S(stream)>>>(A);
   CUDA_OK(cudaGetLastError());
+  return 0;
+}
+extern "C" int evab_expand_cipher_uniform(evab_ctx *c, int n, const uint8_t *seeds, uint64_t *const *c1, const int *ell, const uint64_t *moduli, void *stream) {
+  if (n < 1 || n > 65535) return fail("evab_expand_cipher_uniform: n must be in [1, 65535]");
+  if (!seeds) return fail("evab_expand_cipher_uniform: h_seeds is null");
+  if (!c1) return fail("evab_expand_cipher_uniform: h_c1 is null");
+  if (!ell) return fail("evab_expand_cipher_uniform: h_ell is null");
+  if (!moduli) return fail("evab_expand_cipher_uniform: h_moduli is null");
+  if (c->v.k < 2 || c->v.k > KX_MAXK) return fail("evab_expand_cipher_uniform: 2 <= k <= 64 primes");
+  int maxEll = 0;
+  for (int i = 0; i < n; i++) {
+    if (ell[i] < 1 || ell[i] > c->v.k - 1)
+      return fail("evab_expand_cipher_uniform: h_ell[" + std::to_string(i) + "] must be in [1, k-1] (k = " + std::to_string(c->v.k) + ")");
+    if (!c1[i]) return fail("evab_expand_cipher_uniform: h_c1[" + std::to_string(i) + "] is null");
+    if (reinterpret_cast<uintptr_t>(c1[i]) % 16) return fail("evab_expand_cipher_uniform: h_c1[" + std::to_string(i) + "] is not 16-byte aligned");
+    maxEll = std::max(maxEll, ell[i]);
+  }
+  CipherExpandArgs A{};
+  A.N = (uint32_t)c->v.N;
+  for (int m = 0; m < maxEll; m++) {
+    if (moduli[m] < 2) return fail("evab_expand_cipher_uniform: every modulus in h_moduli must be >= 2");
+    A.q[m] = moduli[m]; A.lim[m] = kx_limit(moduli[m]);
+  }
+  CUDA_OK(cudaSetDevice(c->device));
+  // the entries travel by value in the launch arguments (no device table to keep alive): CX_MAX_ENTRIES per launch, in order on
+  // the caller's stream
+  for (int i0 = 0; i0 < n; i0 += CX_MAX_ENTRIES) {
+    const int nb = std::min(CX_MAX_ENTRIES, n - i0);
+    int rows = 0;
+    for (int b = 0; b < nb; b++) {
+      std::memcpy(A.e[b].seed, seeds + (size_t)32 * (i0 + b), 32);
+      A.e[b].c1 = c1[i0 + b]; A.e[b].ell = (uint32_t)ell[i0 + b];
+      rows = std::max(rows, ell[i0 + b]);
+    }
+    c->launches.fetch_add(1, std::memory_order_relaxed);
+    k_expand_cipher_uniform<<<dim3((A.N / 8 + 255) / 256, rows, nb), 256, 0, S(stream)>>>(A);
+    CUDA_OK(cudaGetLastError());
+  }
   return 0;
 }

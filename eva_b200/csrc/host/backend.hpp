@@ -9,6 +9,7 @@
 #include "executor.hpp"
 #include "slot_cache.hpp"
 #include <atomic>
+#include <functional>
 #include <mutex>
 #include <tuple>
 #include <variant>
@@ -38,7 +39,10 @@ using Valuation = std::map<std::string, std::vector<double>>;
 // host images of ciphertexts / plaintexts live in page-locked memory (asynchronous, full-rate H2D / D2H)
 struct HostCipher { HostBuf data; int size = 0, ell = 0; double scale = 0; };
 struct HostPlain { HostBuf data; int ell = 0; double scale = 0; };
-using SchemeValue = std::variant<HostCipher, HostPlain, std::shared_ptr<ConstantValue>>;
+// a seed-compressed fresh ciphertext (B200Secret::encrypt): c0 [ell][N] and the seed of c1 (key_expand.cuh, ciphertext rows);
+// always size 2.  A type of its own, so that no reader of HostCipher can take its ell N words for 2 ell N
+struct HostSeededCipher { HostBuf c0; int ell = 0; double scale = 0; KeySeed seed{}; };
+using SchemeValue = std::variant<HostCipher, HostPlain, std::shared_ptr<ConstantValue>, HostSeededCipher>;
 
 class B200Valuation {
 public:
@@ -168,6 +172,41 @@ struct Shared {
   std::vector<int> slotsFor(const std::vector<int> &tenants) { return pager ? pager->resolve(tenants) : tenants; }
 };
 
+// SEALPublic::encrypt's checks, slot replication and encoding (reference eva/seal/seal.cpp:24-102), shared by the public-key
+// (B200Public) and the secret-key (B200Secret) encryption: Raw inputs are kept, Plain inputs encoded, and every Cipher input's
+// device plaintext [ell][N] is handed to `cipher`
+inline B200Valuation encodeInputs(Shared &s, const Valuation &inputs, const CKKSSignature &sig,
+                                  const std::function<SchemeValue(const u64 *d_pt, int ell, double scale)> &cipher) {
+  auto &enc = s.client->encoder();
+  const std::size_t slots = enc.slotCount();
+  if (slots < (std::size_t)sig.vecSize) throw std::runtime_error("Vector size cannot be larger than slot count");
+  if (slots % sig.vecSize) throw std::runtime_error("Vector size must exactly divide the slot count");
+  B200Valuation out;
+  const u64 N = s.dev->N();
+  for (auto &in : inputs) {
+    const auto &v = in.second;
+    if (v.size() != (std::size_t)sig.vecSize) throw std::runtime_error("Input size does not match program vector size");
+    const CKKSEncodingInfo &info = sig.inputs.at(in.first);
+    if (info.inputType == Type::Raw) { out[in.first] = std::make_shared<ConstantValue>(sig.vecSize, v); continue; }
+    const int ell = s.dev->k() - 1 - info.level;
+    if (ell < 1) throw std::runtime_error("input level exceeds the modulus chain");
+    std::vector<double> rep;
+    rep.reserve(slots);
+    for (std::size_t r = slots / v.size(); r > 0; --r) rep.insert(rep.end(), v.begin(), v.end());
+    const double scale = std::ldexp(1.0, info.scale);
+    DBuf pt(s.dev, (std::size_t)ell * N);
+    enc.encode(rep, scale, ell, pt.get());
+    if (info.inputType == Type::Cipher) {
+      out[in.first] = cipher(pt.get(), ell, scale);
+    } else {
+      HostPlain h; h.ell = ell; h.scale = scale; h.data.resize((std::size_t)ell * N);
+      s.dev->download(h.data.data(), pt.get(), h.data.size() * 8); s.dev->sync();
+      out[in.first] = std::move(h);
+    }
+  }
+  return out;
+}
+
 // the cached plan of one (program, context) pair; owned by the Program
 struct PlanHolder {
   std::shared_ptr<Shared> keepAlive;  // the plan references the context's encoder and keys
@@ -200,37 +239,12 @@ public:
 
   // SEALPublic::encrypt -- reference eva/seal/seal.cpp:24-102
   B200Valuation encrypt(const Valuation &inputs, const CKKSSignature &sig) {
-    auto &enc = s_->client->encoder();
-    const std::size_t slots = enc.slotCount();
-    if (slots < (std::size_t)sig.vecSize) throw std::runtime_error("Vector size cannot be larger than slot count");
-    if (slots % sig.vecSize) throw std::runtime_error("Vector size must exactly divide the slot count");
-    B200Valuation out;
-    const u64 N = s_->dev->N();
-    for (auto &in : inputs) {
-      const auto &v = in.second;
-      if (v.size() != (std::size_t)sig.vecSize) throw std::runtime_error("Input size does not match program vector size");
-      const CKKSEncodingInfo &info = sig.inputs.at(in.first);
-      if (info.inputType == Type::Raw) { out[in.first] = std::make_shared<ConstantValue>(sig.vecSize, v); continue; }
-      const int ell = s_->dev->k() - 1 - info.level;
-      if (ell < 1) throw std::runtime_error("input level exceeds the modulus chain");
-      std::vector<double> rep;
-      rep.reserve(slots);
-      for (std::size_t r = slots / v.size(); r > 0; --r) rep.insert(rep.end(), v.begin(), v.end());
-      const double scale = std::ldexp(1.0, info.scale);
-      DBuf pt(s_->dev, (std::size_t)ell * N);
-      enc.encode(rep, scale, ell, pt.get());
-      if (info.inputType == Type::Cipher) {
-        DBuf ct = s_->client->encrypt(s_->keys, pt.get(), ell);
-        HostCipher h; h.size = 2; h.ell = ell; h.scale = scale; h.data.resize((std::size_t)2 * ell * N);
-        s_->dev->download(h.data.data(), ct.get(), h.data.size() * 8); s_->dev->sync();
-        out[in.first] = std::move(h);
-      } else {
-        HostPlain h; h.ell = ell; h.scale = scale; h.data.resize((std::size_t)ell * N);
-        s_->dev->download(h.data.data(), pt.get(), h.data.size() * 8); s_->dev->sync();
-        out[in.first] = std::move(h);
-      }
-    }
-    return out;
+    return encodeInputs(*s_, inputs, sig, [&](const u64 *pt, int ell, double scale) -> SchemeValue {
+      DBuf ct = s_->client->encrypt(s_->keys, pt, ell);
+      HostCipher h; h.size = 2; h.ell = ell; h.scale = scale; h.data.resize((std::size_t)2 * ell * s_->dev->N());
+      s_->dev->download(h.data.data(), ct.get(), h.data.size() * 8); s_->dev->sync();
+      return h;
+    });
   }
 
   // one plan (arena, streams, captured graph) per (context, batch, replica); replicas of the same
@@ -258,29 +272,45 @@ public:
   }
   void dropExecutor(Program &program, int batch = 1, int replica = 0) { program.attach(planKey(batch, replica), nullptr); }
 
-  // upload host inputs into the executor's arena (H2D on `stream`).  Client-supplied valuations are untrusted
-  // (they may come from a file): every buffer is checked against the shape the plan expects before any copy.
-  void stageInputs(Executor &ex, Program &program, const B200Valuation &inputs, void *stream, int b = 0) {
+  // upload the host inputs of a chunk's nb valuations into the executor's arena (instance b from inputs[b]; H2D on `stream`).
+  // Client-supplied valuations are untrusted (they may come from a file): every buffer is checked against the shape the plan
+  // expects before its copy.  A seeded ciphertext's c0 is uploaded like any other input; the c1 rows of all of the chunk's seeded
+  // ciphertexts are then expanded on the device by one evab_expand_cipher_uniform call.
+  void stageInputs(Executor &ex, Program &program, const B200Valuation *const *inputs, int nb, void *stream) {
     const u64 N = s_->dev->N();
-    for (auto &in : inputs) {
-      auto term = program.getInput(in.first);
-      const ValueInfo &vi = ex.info(term);
-      if (auto *c = std::get_if<HostCipher>(&in.second)) {
-        if (vi.kind != Kind::Cipher || c->ell != vi.ell || c->size != vi.size || c->data.size() != (std::size_t)vi.size * vi.ell * N)
-          throw std::runtime_error("input " + in.first + ": ciphertext does not match the program signature");
-        s_->dev->upload(ex.valuePtr(term, b), c->data.data(), c->data.size() * 8, stream);
-      } else if (auto *p = std::get_if<HostPlain>(&in.second)) {
-        if (vi.kind != Kind::Plain || p->ell != vi.ell || p->data.size() != (std::size_t)vi.ell * N)
-          throw std::runtime_error("input " + in.first + ": plaintext does not match the program signature");
-        s_->dev->upload(ex.valuePtr(term, b), p->data.data(), (std::size_t)p->ell * N * 8, stream);
-      } else {
-        if (vi.kind != Kind::Raw) throw std::runtime_error("input " + in.first + ": raw vector does not match the program signature");
-        auto &cv = std::get<std::shared_ptr<ConstantValue>>(in.second);
-        std::vector<double> x;
-        cv->expandTo(x, program.getVecSize());
-        ex.setRawInput(in.first, x, b);
+    std::vector<KeySeed> seeds;
+    std::vector<u64 *> c1;
+    std::vector<int> ells;
+    for (int b = 0; b < nb; b++)
+      for (auto &in : *inputs[b]) {
+        auto term = program.getInput(in.first);
+        const ValueInfo &vi = ex.info(term);
+        if (auto *c = std::get_if<HostCipher>(&in.second)) {
+          if (vi.kind != Kind::Cipher || c->ell != vi.ell || c->size != vi.size || c->data.size() != (std::size_t)vi.size * vi.ell * N)
+            throw std::runtime_error("input " + in.first + ": ciphertext does not match the program signature");
+          s_->dev->upload(ex.valuePtr(term, b), c->data.data(), c->data.size() * 8, stream);
+        } else if (auto *sc = std::get_if<HostSeededCipher>(&in.second)) {
+          if (vi.kind != Kind::Cipher || vi.size != 2 || sc->ell != vi.ell || sc->c0.size() != (std::size_t)vi.ell * N)
+            throw std::runtime_error("input " + in.first + ": seeded ciphertext does not match the program signature");
+          u64 *dst = ex.valuePtr(term, b);
+          s_->dev->upload(dst, sc->c0.data(), sc->c0.size() * 8, stream);
+          seeds.push_back(sc->seed); c1.push_back(dst + sc->c0.size()); ells.push_back(sc->ell);
+        } else if (auto *p = std::get_if<HostPlain>(&in.second)) {
+          if (vi.kind != Kind::Plain || p->ell != vi.ell || p->data.size() != (std::size_t)vi.ell * N)
+            throw std::runtime_error("input " + in.first + ": plaintext does not match the program signature");
+          s_->dev->upload(ex.valuePtr(term, b), p->data.data(), (std::size_t)p->ell * N * 8, stream);
+        } else {
+          if (vi.kind != Kind::Raw) throw std::runtime_error("input " + in.first + ": raw vector does not match the program signature");
+          auto &cv = std::get<std::shared_ptr<ConstantValue>>(in.second);
+          std::vector<double> x;
+          cv->expandTo(x, program.getVecSize());
+          ex.setRawInput(in.first, x, b);
+        }
       }
-    }
+    // One launch for the chunk, on the chunk's stream, before its run.  Stream order gives the rest: the expansion starts after the
+    // replica's previous run has stopped reading the arena, a collect() redo (the zero-digit case) stages again and so expands the
+    // same words again, and a packed arena never lends an input's storage to another value (inputs are pinned).
+    if (!seeds.empty()) expandCiphers(*s_->dev, (int)seeds.size(), seeds.data(), c1.data(), ells.data(), stream);
   }
   // plans and arenas are cached on the Program: a call that omits an input would silently compute on the previous
   // call's ciphertext.  The reference builds a fresh executor per call and fails on the missing value
@@ -396,7 +426,7 @@ public:
       if (std::find(streams.begin(), streams.end(), st) == streams.end()) streams.push_back(st);
       if (std::find(p.plans.begin(), p.plans.end(), holder) == p.plans.end()) p.plans.push_back(holder);
       auto t1 = now();
-      for (int b = 0; b < nb; b++) stageInputs(ex, program, *inputs[b0 + b], st, b);
+      stageInputs(ex, program, inputs.data() + b0, nb, st);
       auto t2 = now();
       if (pager) pager->beforeRun(st, slots.data() + b0, nb);
       ex.run(st);
@@ -498,7 +528,9 @@ public:
     Executor &ex = pub_->executorFor(prog, (int)rq.size(), replica);
     staged_[&ex] = tenants;
     setSlots(ex, shared()->slotsFor(tenants), stream);
-    for (std::size_t b = 0; b < rq.size(); b++) pub_->stageInputs(ex, prog, *rq[b].second, stream, (int)b);
+    std::vector<const B200Valuation *> in;
+    for (auto &r : rq) in.push_back(r.second);
+    pub_->stageInputs(ex, prog, in.data(), (int)in.size(), stream);
   }
   // tenants: replaces the staged tenants of the replica (same count)
   void runResident(Program &prog, void *stream, int batch, int replica, const std::vector<int> &tenants = {}) {
@@ -548,6 +580,17 @@ private:
 class B200Secret {
 public:
   explicit B200Secret(std::shared_ptr<Shared> s) : s_(std::move(s)) {}
+  // Encryptor::encrypt_symmetric (SEAL's seed-compressed Serializable<Ciphertext>): B200Public::encrypt's checks and encoding, every
+  // Cipher input a seeded ciphertext (c0 and the seed of c1, half the bytes).  Only the holder of the secret key can make one
+  B200Valuation encrypt(const Valuation &inputs, const CKKSSignature &sig) {
+    if (!s_->keys.sk) throw std::runtime_error("this context has no secret key");
+    return encodeInputs(*s_, inputs, sig, [&](const u64 *pt, int ell, double scale) -> SchemeValue {
+      auto ct = s_->client->encryptSeeded(s_->keys, pt, ell);
+      HostSeededCipher h; h.ell = ell; h.scale = scale; h.seed = ct.second; h.c0.resize((std::size_t)ell * s_->dev->N());
+      s_->dev->download(h.c0.data(), ct.first.get(), h.c0.size() * 8); s_->dev->sync();
+      return h;
+    });
+  }
   // SEALSecret::decrypt -- reference eva/seal/seal.cpp:124-146
   Valuation decrypt(const B200Valuation &enc, const CKKSSignature &sig) {
     Valuation out;
@@ -559,6 +602,16 @@ public:
         s_->dev->upload(ct.get(), c->data.data(), c->data.size() * 8);
         DBuf pt = s_->client->decrypt(s_->keys, ct.get(), c->size, c->ell);
         out[e.first] = encoder.decode(pt.get(), c->ell, c->scale);
+      } else if (auto *sc = std::get_if<HostSeededCipher>(&e.second)) {
+        // c1 expanded from the seed on the device, then decrypted as a full ciphertext
+        if (sc->ell < 1 || sc->ell > s_->dev->k() - 1 || sc->c0.size() != (std::size_t)sc->ell * N)
+          throw std::runtime_error("value " + e.first + ": seeded ciphertext does not match the parameters (level / degree)");
+        DBuf ct(s_->dev, 2 * sc->c0.size());
+        s_->dev->upload(ct.get(), sc->c0.data(), sc->c0.size() * 8);
+        u64 *c1 = ct.get() + sc->c0.size();
+        expandCiphers(*s_->dev, 1, &sc->seed, &c1, &sc->ell, nullptr);
+        DBuf pt = s_->client->decrypt(s_->keys, ct.get(), 2, sc->ell);
+        out[e.first] = encoder.decode(pt.get(), sc->ell, sc->scale);
       } else if (auto *p = std::get_if<HostPlain>(&e.second)) {
         DBuf pt(s_->dev, (std::size_t)p->ell * N);
         s_->dev->upload(pt.get(), p->data.data(), (std::size_t)p->ell * N * 8);

@@ -222,6 +222,12 @@ inline void expandKeys(Device &dev, int n, const u64 *d_seeds, u64 *d_keys, void
   check(evab_expand_key_uniform(dev.ctx(), n, reinterpret_cast<const std::uint8_t *>(d_seeds), dev.primes().data(), d_keys, stream));
 }
 
+// the c1 rows of n seed-compressed ciphertexts: entry i writes ell[i] rows at the device pointer c1[i] from seeds[i], modulo the
+// context's primes (key_expand.cuh, ciphertext rows); stream-ordered
+inline void expandCiphers(Device &dev, int n, const KeySeed *seeds, u64 *const *c1, const int *ell, void *stream) {
+  check(evab_expand_cipher_uniform(dev.ctx(), n, reinterpret_cast<const std::uint8_t *>(seeds), c1, ell, dev.primes().data(), stream));
+}
+
 // a full key-switch key on the device from its compressed form: host c0 rows [k-1][k][N] and the seed
 inline DBuf expandCompressedKey(const std::shared_ptr<Device> &dev, const u64 *c0, const KeySeed &seed) {
   const std::size_t kN = (std::size_t)dev->k() * dev->N();
@@ -302,6 +308,32 @@ public:
     DBuf work(dev_, evab_rescale_work_bytes(dev_->ctx(), 2) / 8);
     check(evab_rescale(dev_->ctx(), nres, ct.get(), big.get(), 2, work.get(), nullptr));
     check(evab_add_plain(dev_->ctx(), ell, ct.get(), ct.get(), 2, d_pt, nullptr));
+    dev_->sync();
+    return ct;
+  }
+  // Encryptor::encrypt_symmetric with a seed-compressed result; d_pt[ell][N].  Draws, in this order: a fresh 32-byte seed (4 words of
+  // the client's stream), then the error e (sampleCbd, N words).  Returns ct [2][ell][N] and the seed; only c0 (the first ell N
+  // words) has to travel, c1 is the seed's expansion
+  std::pair<DBuf, KeySeed> encryptSeeded(const KeySet &K, const u64 *d_pt, int ell) {
+    const KeySeed seed = drawSeed();
+    const std::vector<int> e = sampleCbd();
+    return {encryptSeededWith(K, d_pt, ell, seed, e), seed};
+  }
+  // the deterministic core (also a test hook): c1 = a expanded from `seed` on the device, c0 = -(a s + e) + pt on the first ell
+  // residues of s.  No special-prime lift: the encryption is made at its level, as SEAL's symmetric path does
+  DBuf encryptSeededWith(const KeySet &K, const u64 *d_pt, int ell, const KeySeed &seed, const std::vector<int> &e) {
+    if (!K.sk) throw std::runtime_error("secret-key encryption needs the secret key: this context has none");
+    if (ell < 1 || ell > k_ - 1) throw std::invalid_argument("encryption level out of range");
+    if (e.size() != N_) throw std::invalid_argument("the error must have N entries");
+    const std::size_t P = (std::size_t)ell * N_;
+    DBuf ct(dev_, 2 * P);
+    u64 *c0 = ct.get(), *c1 = ct.get() + P;
+    expandCiphers(*dev_, 1, &seed, &c1, &ell, nullptr);
+    DBuf ed = smallToDeviceNtt(e, ell);
+    check(evab_mul_plain(dev_->ctx(), ell, c0, c1, 1, K.sk.get(), nullptr));
+    check(evab_add_plain(dev_->ctx(), ell, c0, c0, 1, ed.get(), nullptr));
+    check(evab_negate(dev_->ctx(), ell, c0, c0, 1, nullptr));
+    check(evab_add_plain(dev_->ctx(), ell, c0, c0, 1, d_pt, nullptr));
     dev_->sync();
     return ct;
   }

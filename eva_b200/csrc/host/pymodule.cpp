@@ -37,6 +37,21 @@ static KeySeed toSeed(const py::bytes &b, const char *what) {
 }
 static py::bytes fromSeed(const KeySeed &s) { return py::bytes(reinterpret_cast<const char *>(s.data()), 32); }
 
+// test hook of B200Public / B200Secret: Encryptor::encrypt_symmetric of a plaintext polynomial [ell][N] with an EXPLICIT seed and
+// error -> the full ciphertext [2][ell][N] (c1: the seed's expansion)
+static u64arr encryptSeededPoly(const std::shared_ptr<Shared> &s, const u64arr &pt, const py::bytes &seed, const std::vector<int> &e) {
+  if (pt.ndim() != 2 || (std::size_t)pt.shape(1) != s->dev->N()) throw std::runtime_error("plaintext array must be [ell][N]");
+  const KeySeed sd = toSeed(seed, "ciphertext");
+  const int ell = (int)pt.shape(0);
+  DBuf d(s->dev, pt.size());
+  s->dev->upload(d.get(), pt.data(), pt.size() * 8);
+  DBuf ct = s->client->encryptSeededWith(s->keys, d.get(), ell, sd, e);
+  u64arr a({(std::size_t)2, (std::size_t)ell, (std::size_t)s->dev->N()});
+  s->dev->download(a.mutable_data(), ct.get(), a.size() * 8);
+  s->dev->sync();
+  return a;
+}
+
 // set_options: one argument list for B200Public and for the planner test hook (_plan), which parses its options dict through it
 static ExecOptions &optionsOf(B200Public &p) { return p.options; }
 static ExecOptions &optionsOf(B200Server &s) { return s.pub().options; }
@@ -247,6 +262,17 @@ PYBIND11_MODULE(_eva_b200, m) {
         HostCipher h; h.data = toHostBuf(data); h.size = (int)data.shape(0); h.ell = (int)data.shape(1); h.scale = scale;
         v[name] = std::move(h);
       }, "test/benchmark hook: inject a raw ciphertext [size][ell][N]")
+      .def("set_seeded_cipher", [](B200Valuation &v, const std::string &name, const u64arr &c0, const py::bytes &seed, double scale) {
+        if (c0.ndim() != 2) throw std::runtime_error("seeded ciphertext c0 must be [ell][N]");
+        HostSeededCipher h; h.seed = toSeed(seed, "ciphertext"); h.c0 = toHostBuf(c0); h.ell = (int)c0.shape(0); h.scale = scale;
+        v[name] = std::move(h);
+      }, py::arg("name"), py::arg("c0"), py::arg("seed"), py::arg("scale"),
+         "a seed-compressed fresh ciphertext (B200Secret.encrypt): c0 [ell][N] and the 32-byte seed from which c1 is expanded")
+      .def("get_seed", [](const B200Valuation &v, const std::string &name) {
+        auto *sc = std::get_if<HostSeededCipher>(&v.at(name));
+        if (!sc) throw std::invalid_argument("value " + name + " is not a seeded ciphertext");
+        return fromSeed(sc->seed);
+      }, py::arg("name"), "the 32-byte seed of a seeded ciphertext")
       .def("set_plain", [](B200Valuation &v, const std::string &name, const u64arr &data, double scale) {
         if (data.ndim() != 2) throw std::runtime_error("plaintext array must be [ell][N]");
         HostPlain h; h.data = toHostBuf(data); h.ell = (int)data.shape(0); h.scale = scale; v[name] = std::move(h);
@@ -265,6 +291,12 @@ PYBIND11_MODULE(_eva_b200, m) {
           u64arr a({(std::size_t)p->ell, N});
           std::memcpy(a.mutable_data(), p->data.data(), p->data.size() * 8);
           return py::make_tuple("plain", a, p->scale);
+        }
+        if (auto *sc = std::get_if<HostSeededCipher>(&sv)) {   // c0 only (the seed: get_seed)
+          const std::size_t N = sc->c0.size() / (std::size_t)sc->ell;
+          u64arr a({(std::size_t)sc->ell, N});
+          std::memcpy(a.mutable_data(), sc->c0.data(), sc->c0.size() * 8);
+          return py::make_tuple("seeded_cipher", a, sc->scale);
         }
         return py::make_tuple("raw", std::get<std::shared_ptr<ConstantValue>>(sv)->values(), 0.0);
       });
@@ -331,7 +363,7 @@ PYBIND11_MODULE(_eva_b200, m) {
       // ---- benchmark hooks: device-resident execution on a caller-provided stream
       .def("stage_inputs", [](B200Public &p, Program &prog, const std::vector<const B200Valuation *> &in, std::uintptr_t stream, int replica) {
         Executor &ex = p.executorFor(prog, (int)in.size(), replica);
-        for (std::size_t b = 0; b < in.size(); b++) p.stageInputs(ex, prog, *in[b], (void *)stream, (int)b);
+        p.stageInputs(ex, prog, in.data(), (int)in.size(), (void *)stream);
       }, py::arg("program"), py::arg("inputs"), py::arg("stream"), py::arg("replica") = 0)
       .def("run_resident", [](B200Public &p, Program &prog, std::uintptr_t stream, int batch, int replica) { p.executorFor(prog, batch, replica).run((void *)stream); },
            py::arg("program"), py::arg("stream"), py::arg("batch") = 1, py::arg("replica") = 0, py::call_guard<py::gil_scoped_release>())
@@ -410,6 +442,9 @@ PYBIND11_MODULE(_eva_b200, m) {
         s->dev->sync();
         return a;
       }, py::arg("plaintext"), py::arg("u"), py::arg("e0"), py::arg("e1"))
+      .def("encrypt_seeded_poly", [](B200Public &p, const u64arr &pt, const py::bytes &seed, const std::vector<int> &e) {
+        return encryptSeededPoly(p.shared(), pt, seed, e);
+      }, py::arg("plaintext"), py::arg("seed"), py::arg("e"), "test hook (contexts that hold the secret key): secret-key encryption with an explicit seed and error")
       .def("decode", [](B200Public &p, const u64arr &pt, double scale) {
         auto dev = p.shared()->dev;
         DBuf d(dev, pt.size());
@@ -417,8 +452,14 @@ PYBIND11_MODULE(_eva_b200, m) {
         return p.shared()->client->encoder().decode(d.get(), (int)pt.shape(0), scale);
       });
   defSetOptions(pub);
-  py::class_<B200Secret>(mb, "B200Secret","The secret part of the context: decryption")
+  py::class_<B200Secret>(mb, "B200Secret","The secret part of the context: decryption, and secret-key encryption of compact inputs")
       .def("decrypt", &B200Secret::decrypt, py::arg("enc_outputs"), py::arg("signature"))
+      .def("encrypt", &B200Secret::encrypt, py::arg("inputs"), py::arg("signature"),
+           "B200Public.encrypt with the secret key: every Cipher input becomes a seeded ciphertext (c0 and a 32-byte seed, half the bytes); "
+           "Plain and Raw inputs as B200Public.encrypt makes them")
+      .def("encrypt_seeded_poly", [](B200Secret &x, const u64arr &pt, const py::bytes &seed, const std::vector<int> &e) {
+        return encryptSeededPoly(x.shared(), pt, seed, e);
+      }, py::arg("plaintext"), py::arg("seed"), py::arg("e"), "test hook: secret-key encryption with an explicit seed and error -> [2][ell][N]")
       // test hook: Decryptor::decrypt of a raw ciphertext [size][ell][N] -> plaintext polynomial [ell][N] (before decoding)
       .def("decrypt_poly", [](B200Secret &x, const u64arr &ct) {
         auto s = x.shared();

@@ -1,4 +1,5 @@
-// key_expand.cuh -- the uniform halves of seed-compressed key-switch keys (DESIGN §2, "Seed-compressed evaluation keys").
+// key_expand.cuh -- the uniform halves of seed-compressed key-switch keys (DESIGN §2, "Seed-compressed evaluation keys") and of
+// seed-compressed input ciphertexts (the same rule with other row ids, at the end of this file).
 //
 // Digit J of a key-switch key [k-1][2][k][N] is (c0, c1) = (-(a s + e) + P [J] s', a), where a is uniform public randomness.  A
 // compressed key keeps c0 and a 32-byte seed; its (k-1) k rows of c1 are rebuilt from the seed alone by this rule:
@@ -14,7 +15,8 @@
 //                                in order and takes the first accepted one (all 2048 rejected, probability < 2^-2048: the last
 //                                candidate mod q)
 // Each coefficient depends on (seed, r, j) only, so a key expands in one parallel pass.  The block function is also the host
-// CSPRNG's (host/csprng.hpp), and tests/emu/emu_expand.cpp replays this file on the CPU.
+// CSPRNG's (host/csprng.hpp), and tests/emu/emu_expand.cpp (key rows) and tests/emu/emu_cipher_expand.cpp (ciphertext rows) replay
+// this file on the CPU.
 #pragma once
 #include <stddef.h>
 #include <stdint.h>
@@ -65,7 +67,7 @@ struct ExpandArgs {
 };
 
 // coefficient j of row r, rejected in the primary draw: the fallback search
-EVAB_HD uint64_t kx_fallback(const uint32_t *key, uint64_t q, uint64_t lim, uint32_t r, uint32_t j) {
+EVAB_HD uint64_t kx_fallback(const uint32_t *key, uint64_t q, uint64_t lim, uint64_t r, uint32_t j) {
   uint32_t w[16];
   uint64_t v = 0;
   for (uint32_t t = 0; t < KX_FALLBACK_BLOCKS; t++) {
@@ -78,6 +80,29 @@ EVAB_HD uint64_t kx_fallback(const uint32_t *key, uint64_t q, uint64_t lim, uint
   return v % q;
 }
 
+// the rule's draw, shared by key rows and ciphertext rows: coefficients 8 t .. 8 t + 7 of row r (modulus q, lim = kx_limit(q))
+// from one primary block, a rejected candidate replaced by its fallback search
+EVAB_HD void kx_draw8(const uint32_t *key, uint64_t r, uint32_t t, uint64_t q, uint64_t lim, uint64_t *v) {
+  uint32_t w[16];
+  chacha20_block(key, t, r, w);
+#pragma unroll
+  for (int i = 0; i < 8; i++) {
+    const uint64_t c = (uint64_t)w[2 * i] | ((uint64_t)w[2 * i + 1] << 32);
+    v[i] = c < lim ? c % q : kx_fallback(key, q, lim, r, 8 * t + i);
+  }
+}
+
+// 8 coefficients to dst (64-byte aligned: N is a multiple of 8 and rows start on 64-byte boundaries): 16-byte stores on the device
+EVAB_HD void kx_store8(uint64_t *dst, const uint64_t *v) {
+#if defined(__CUDA_ARCH__)
+  ulonglong2 *d2 = reinterpret_cast<ulonglong2 *>(dst);
+#pragma unroll
+  for (int i = 0; i < 4; i++) d2[i] = make_ulonglong2(v[2 * i], v[2 * i + 1]);
+#else
+  for (int i = 0; i < 8; i++) dst[i] = v[i];
+#endif
+}
+
 // key g, row r, coefficients 8 t .. 8 t + 7: one primary block
 EVAB_HD void expand_uniform_elem(const ExpandArgs &A, uint32_t g, uint32_t r, uint32_t t) {
   uint32_t key[8];
@@ -85,21 +110,41 @@ EVAB_HD void expand_uniform_elem(const ExpandArgs &A, uint32_t g, uint32_t r, ui
 #pragma unroll
   for (int i = 0; i < 8; i++) key[i] = sk[i];
   const uint32_t J = r / A.k, m = r % A.k;
-  const uint64_t q = A.q[m], lim = A.lim[m];
-  uint32_t w[16];
-  chacha20_block(key, t, r, w);
   uint64_t v[8];
-#pragma unroll
-  for (int i = 0; i < 8; i++) {
-    const uint64_t c = (uint64_t)w[2 * i] | ((uint64_t)w[2 * i + 1] << 32);
-    v[i] = c < lim ? c % q : kx_fallback(key, q, lim, r, 8 * t + i);
-  }
-  uint64_t *dst = A.keys + (size_t)g * (A.k - 1) * 2 * A.k * A.N + ((size_t)(2 * J + 1) * A.k + m) * A.N + (size_t)8 * t;
-#if defined(__CUDA_ARCH__)
-  ulonglong2 *d2 = reinterpret_cast<ulonglong2 *>(dst);   // 64-byte aligned: N is a multiple of 8
-#pragma unroll
-  for (int i = 0; i < 4; i++) d2[i] = make_ulonglong2(v[2 * i], v[2 * i + 1]);
-#else
-  for (int i = 0; i < 8; i++) dst[i] = v[i];
+  kx_draw8(key, r, t, A.q[m], A.lim[m], v);
+  kx_store8(A.keys + (size_t)g * (A.k - 1) * 2 * A.k * A.N + ((size_t)(2 * J + 1) * A.k + m) * A.N + (size_t)8 * t, v);
+}
+
+// ---- seed-compressed ciphertexts (DESIGN §2, "Seed-compressed input ciphertexts").  A fresh secret-key encryption
+// (c0, c1) = (-(a s + e) + m, a) at level ell keeps c0 and a 32-byte seed; its ell rows of c1 follow the same rule with their own
+// row ids:
+//   row id of ciphertext row m   r = 2^62 | m (prime index m < ell, modulus q_m); key rows are r = J k + m < 2^12, so a key and
+//                                a ciphertext never share a ChaCha stream, even under the same seed.  The fallback nonce is
+//                                2^63 | r as for keys
+//   primary draw                 coefficient j of row m takes candidate j mod 8 of block(seed, j / 8, 2^62 | m)
+#define KX_CIPHER_ROW (1ull << 62)
+#define CX_MAX_ENTRIES 56                 // ciphertexts per launch: the arguments stay under 4 KB of kernel parameters
+
+struct CipherExpandEntry {
+  uint32_t seed[8];                       // 32 bytes, as 8 little-endian key words
+  uint64_t *c1;                           // the ell rows [ell][N] of c1 (the ciphertext [2][ell][N] starts ell N words before)
+  uint32_t ell;
+};
+struct CipherExpandArgs {
+  uint64_t q[KX_MAXK], lim[KX_MAXK];      // modulus of prime index m, kx_limit(q)
+  CipherExpandEntry e[CX_MAX_ENTRIES];
+  uint32_t N;
+};
+#if defined(__cplusplus) && __cplusplus >= 201103L
+static_assert(sizeof(CipherExpandArgs) <= 4096, "the ciphertext expansion's arguments must fit the classic 4 KB parameter space");
 #endif
+
+// entry i, row m < e[i].ell, coefficients 8 t .. 8 t + 7
+EVAB_HD void expand_cipher_elem(const CipherExpandArgs &A, uint32_t i, uint32_t m, uint32_t t) {
+  uint32_t key[8];
+#pragma unroll
+  for (int w = 0; w < 8; w++) key[w] = A.e[i].seed[w];
+  uint64_t v[8];
+  kx_draw8(key, KX_CIPHER_ROW | m, t, A.q[m], A.lim[m], v);
+  kx_store8(A.e[i].c1 + (size_t)m * A.N + (size_t)8 * t, v);
 }

@@ -567,6 +567,8 @@ def _subset(inputs, names):
             kind, arr, scale = inputs.get(name)
             if kind == "cipher":
                 out.set_cipher(name, arr, scale)
+            elif kind == "seeded_cipher":      # carried compressed: the instance that stages it expands c1
+                out.set_seeded_cipher(name, arr, inputs.get_seed(name), scale)
             elif kind == "plain":
                 out.set_plain(name, arr, scale)
             else:

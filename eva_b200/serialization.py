@@ -142,6 +142,9 @@ _KEY_OF = {v[0]: k for k, v in _ATTRS.items()}
 # payload kinds (EVAB header only) of seed-compressed keys, under the RELIN_KEYS / GALOIS_KEYS objects: the c0 rows [k-1][k][N] of
 # every key, and in the header's extra words its 32-byte seed as 4 little-endian u64 words (Galois: the elements, then the seeds)
 COMPRESSED_RELIN_KEYS, COMPRESSED_GALOIS_KEYS = 16, 17
+# payload kind of a seed-compressed input ciphertext (B200Secret.encrypt), under the CIPHERTEXT object: c0 [ell][N], and in the
+# header's extra words the 32-byte seed of c1 as 4 little-endian u64 words
+COMPRESSED_CIPHERTEXT = 18
 
 
 # ------------------------------------------------------------------ Program / parameters / signature
@@ -372,6 +375,9 @@ def valuation_to_msg(val):
         if kind == "cipher":
             o = msg.values[name]
             o.seal_type, o.data = CIPHERTEXT, _pack(CIPHERTEXT, arr, scale)
+        elif kind == "seeded_cipher":
+            o = msg.values[name]
+            o.seal_type, o.data = CIPHERTEXT, _pack(COMPRESSED_CIPHERTEXT, arr, scale, extra=_seed_words(val.get_seed(name)))
         elif kind == "plain":
             o = msg.values[name]
             o.seal_type, o.data = PLAINTEXT, _pack(PLAINTEXT, arr, scale)
@@ -386,7 +392,12 @@ def valuation_from_msg(msg):
     from . import b200
     val = b200.B200Valuation()
     for name, o in msg.values.items():
-        if o.seal_type == CIPHERTEXT:
+        if o.seal_type == CIPHERTEXT and _kind(o.data) == COMPRESSED_CIPHERTEXT:
+            arr, scale, words = _unpack(o.data, COMPRESSED_CIPHERTEXT)
+            if len(words) != 4:
+                raise RuntimeError("compressed ciphertext %s: the seed must be 32 bytes" % name)
+            val.set_seeded_cipher(name, arr, _seed_bytes(words), scale)
+        elif o.seal_type == CIPHERTEXT:
             arr, scale, _ = _unpack(o.data, CIPHERTEXT)
             val.set_cipher(name, arr, scale)
         else:

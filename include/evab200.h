@@ -222,6 +222,15 @@ int evab_rotate_hoist_const_levels(evab_ctx *ctx, int n, const uint64_t *galois_
  * h_moduli[m] (host array of the k moduli, read during the call; the context's primes for real keys, any moduli >= 2 for
  * tests).  The c0 rows are not touched.  One launch; stream-ordered, does not synchronise.  1 <= n <= 65535, k <= 64. */
 int evab_expand_key_uniform(evab_ctx *ctx, int n, const uint8_t *d_seeds, const uint64_t *h_moduli, uint64_t *d_keys, void *stream);
+/* Seed-compressed input ciphertexts: the c1 rows of n fresh secret-key encryptions (c0, c1) = (-(a s + e) + m, a), expanded from
+ * their 32-byte seeds by the same rule with the row ids 2^62 | m (key_expand.cuh; DESIGN §2).  Entry i writes the ell_i rows
+ * [h_ell[i]][N] at h_c1[i] (a device pointer, 16-byte aligned: the c1 half of a ciphertext [2][ell_i][N] that starts ell_i N words
+ * before) from h_seeds[i] (host, [n][32] bytes), row m modulo h_moduli[m] (host, >= max ell entries; the context's primes for real
+ * ciphertexts, any moduli >= 2 for tests).  Nothing else is written.  The pointers are explicit: evab_set_batch does not apply.
+ * All arrays are read during the call (the entries travel in the launch arguments, up to 56 per launch; larger n is split into
+ * several launches on `stream`).  Stream-ordered, does not synchronise.  1 <= n <= 65535, 1 <= h_ell[i] <= k-1. */
+int evab_expand_cipher_uniform(evab_ctx *ctx, int n, const uint8_t *h_seeds, uint64_t *const *h_c1, const int *h_ell, const uint64_t *h_moduli,
+                               void *stream);
 /* n <= 16 rotations of ONE ciphertext (seal::Evaluator::rotate_vector, seal_executor.h:176-189) in three kernel launches instead of
  * 3 n: d_out [n][2][ell][N], rotation i by galois_elts[i]; same bits as n calls of evab_rotate_modup_prepared.  d_ext, keys, cadds as there. */
 /* evab_rotate_modup_many and evab_lazy_rotsum read P * c0 from the diagonal of d_ext (ext[m][J] has no entry for m = q_J): call this once
