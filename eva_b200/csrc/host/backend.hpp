@@ -34,6 +34,21 @@ struct CKKSSignature {
 };
 using Valuation = std::map<std::string, std::vector<double>>;
 
+// The rotation steps that get a Galois key.  "program": every step of the program (the compiler's rotation set, step 0 included).
+// "power_of_two": the distinct NAF terms of its nonzero steps but those of magnitude N/2, ascending; every rotation of the program
+// is then composed from them as SEAL's rotate_vector does (planner.hpp composeRotations)
+inline std::vector<int> rotationKeySteps(const CKKSParameters &params, const std::string &rotationKeys) {
+  if (rotationKeys == "program") return std::vector<int>(params.rotations.begin(), params.rotations.end());
+  if (rotationKeys != "power_of_two") throw std::invalid_argument("rotation_keys must be \"program\" or \"power_of_two\", not \"" + rotationKeys + "\"");
+  std::set<int> steps;
+  for (int s : params.rotations) {
+    if (!s) continue;
+    if (!evab_host::galois_elt_from_step(params.polyModulusDegree, s)) throw std::invalid_argument("step count too large");
+    for (int t : evab_host::naf_rotation_terms(params.polyModulusDegree, s)) steps.insert(t);
+  }
+  return std::vector<int>(steps.begin(), steps.end());
+}
+
 // host-resident encrypted values (the reference keeps seal::Ciphertext objects
 // in host memory inside SEALValuation, eva/seal/seal.h:21-41)
 // host images of ciphertexts / plaintexts live in page-locked memory (asynchronous, full-rate H2D / D2H)
@@ -477,15 +492,18 @@ private:
 class B200Server {
 public:
   // maxTenants < 0 or == capacity: tenant id = bank region, filled when the keys are added.  maxTenants > capacity: paging (KeyPager)
-  B200Server(const CKKSParameters &params, int capacity, int device, int maxTenants = -1) {
+  // rotationKeys: the bank's Galois keys (rotationKeySteps); rotations without a key of their own are composed
+  B200Server(const CKKSParameters &params, int capacity, int device, int maxTenants = -1, const std::string &rotationKeys = "program")
+      : rotationKeys_(rotationKeys) {
     if (maxTenants >= 0 && maxTenants < capacity)
       throw std::invalid_argument("max_tenants (" + std::to_string(maxTenants) + ") is below the number of device slots (capacity " + std::to_string(capacity) + ")");
+    const std::vector<int> steps = rotationKeySteps(params, rotationKeys);
     std::vector<int> bits(params.primeBits.begin(), params.primeBits.end());
     auto s = std::make_shared<Shared>();
     s->dev = std::make_shared<Device>(params.polyModulusDegree, hmod::createCoeffModulus(params.polyModulusDegree, bits), device);
     s->client = std::make_unique<CkksClient>(s->dev, 0);
     std::set<u64> elts;
-    for (int step : params.rotations) {
+    for (int step : steps) {
       const u64 elt = evab_galois_elt_from_step(params.polyModulusDegree, step);
       if (!elt) throw std::invalid_argument("step count too large");
       elts.insert(elt);
@@ -564,6 +582,7 @@ public:
   }
   B200Public &pub() { return *pub_; }
   const KeyBank &bank() const { return *pub_->shared()->bank; }
+  const std::string &rotationKeys() const { return rotationKeys_; }
   std::shared_ptr<Shared> shared() const { return pub_->shared(); }
 
 private:
@@ -573,6 +592,7 @@ private:
     shared()->dev->sync(stream);
     ex.setTenants(slots.data(), (int)slots.size());
   }
+  std::string rotationKeys_;
   std::unique_ptr<B200Public> pub_;
   std::map<const Executor *, std::vector<int>> staged_;   // device-resident hooks: the tenants staged on a plan replica
 };
@@ -630,7 +650,8 @@ private:
 
 // generateKeys -- reference eva/seal/seal.cpp:174-203
 inline std::tuple<std::unique_ptr<B200Public>, std::unique_ptr<B200Secret>>
-generateKeys(const CKKSParameters &params, int device = 0, std::uint64_t seed = 0) {
+generateKeys(const CKKSParameters &params, int device = 0, std::uint64_t seed = 0, const std::string &rotationKeys = "program") {
+  const std::vector<int> rots = rotationKeySteps(params, rotationKeys);
   std::vector<int> bits(params.primeBits.begin(), params.primeBits.end());
   auto primes = hmod::createCoeffModulus(params.polyModulusDegree, bits);
   auto s = std::make_shared<Shared>();
@@ -638,7 +659,6 @@ generateKeys(const CKKSParameters &params, int device = 0, std::uint64_t seed = 
   // seed == 0 (the default): keys and encryption randomness from a CSPRNG keyed with 256 bits of OS entropy;
   // a non-zero seed is the deterministic test path (host/csprng.hpp)
   s->client = std::make_unique<CkksClient>(s->dev, seed);
-  std::vector<int> rots(params.rotations.begin(), params.rotations.end());
   s->client->keygen(s->keys, rots);
   return std::make_tuple(std::make_unique<B200Public>(s), std::make_unique<B200Secret>(s));
 }

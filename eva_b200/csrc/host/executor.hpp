@@ -240,7 +240,10 @@ private:
     ws.encode = [c](int count) { return evab_encode_work_bytes(c, count); };
     std::size_t limit = opt.arenaLimit;
     if (!limit) { std::size_t freeB = 0, totalB = 0; check(evab_mem_info(dev_->ctx(), &freeB, &totalB)); limit = freeB; }
-    return buildPlan(prog_, opt, dev_->N(), dev_->k(), limit, ws);
+    std::set<u64> elts;   // rotations by steps without a key of their own are composed (planner.hpp composeRotations)
+    if (bank_) elts.insert(bank_->elements().begin(), bank_->elements().end());
+    else for (auto &g : keys_.galois) elts.insert(g.first);
+    return buildPlan(prog_, opt, dev_->N(), dev_->k(), limit, ws, &elts);
   }
   // device side of the plan: arenas, streams, events, plan-time encodes, Galois tables and hoist constants
   void materialise() {
@@ -281,9 +284,9 @@ private:
   const u64 *relinKey() const { return bank_ ? bank_->relin() : keys_.relin.get(); }
   const u64 *galoisKey(u64 elt) const { return bank_ ? bank_->galois(elt) : keys_.galois.at(elt).get(); }
   const u64 *hoistConst(u64 elt, int ell) const { return bank_ ? bank_->hoistConst(elt, ell) : hoistConst_.at(std::make_pair(elt, ell)).get(); }
+  // the element of the rotation a term applies (a hop of a composed rotation: its term's)
   u64 galoisElt(const Term &t) const {
-    const int steps = t.op == Op::RotateLeftConst ? *t.rotation : -*t.rotation;
-    const u64 elt = evab_galois_elt_from_step(N_, steps);
+    const u64 elt = evab_galois_elt_from_step(N_, plan_.stepOf(&t));
     if (!elt) throw std::invalid_argument("step count too large");
     return elt;
   }
@@ -362,7 +365,7 @@ private:
   // named after its term, so that nsys / ncu timelines read in program terms.  EVAB_NVTX=1 gives the ranges alone.
   struct TraceScope {
     bool nvtx;
-    TraceScope(const Step &st, bool print, bool nvtx_) : nvtx(nvtx_) {
+    TraceScope(const Plan &p, const Step &st, bool print, bool nvtx_) : nvtx(nvtx_) {
       if (!print && !nvtx) return;
       char name[96];
       const Term &t = *st.term;
@@ -374,6 +377,7 @@ private:
         std::printf("EVA: Execute t%lu%s = %s(", (unsigned long)t.index, term ? "" : "'", term ? opName(t.op) : pseudo);
         bool first = true;
         if (!term) std::printf("t%lu", (unsigned long)t.index);
+        else if (p.chainSrc.count(t.index)) std::printf("t%lu", (unsigned long)p.src(&t)->index);   // a hop of a composed rotation
         else for (auto &o : t.getOperands()) { std::printf(first ? "t%lu" : ",t%lu", (unsigned long)o->index); first = false; }
         std::printf(")  [stream %d%s]\n", st.stream, st.sum.empty() ? "" : ", fused sum");
         std::fflush(stdout);
@@ -386,7 +390,7 @@ private:
   void issue(const Step &st, void *stream) {
     const Plan &p = plan_;
     const Term &t = *st.term;
-    TraceScope trace(st, verbosity() >= 2, traceNvtx());
+    TraceScope trace(p, st, verbosity() >= 2, traceNvtx());
     evab_ctx *c = dev_->ctx();
     const ValueInfo &o = p.vals[t.index];
     u64 *const A = arena_.get();
@@ -405,7 +409,7 @@ private:
         const RotChunk &ch = p.chunks[st.index];
         if (verbosity() >= 2)
           for (const Term *r : ch.rots)
-            std::printf("EVA: Execute t%lu = %s(t%lu)  [stream %d, in the batch above]\n", (unsigned long)r->index, opName(r->op), (unsigned long)r->operandAt(0)->index, st.stream);
+            std::printf("EVA: Execute t%lu = %s(t%lu)  [stream %d, in the batch above]\n", (unsigned long)r->index, opName(r->op), (unsigned long)(p.chainSrc.count(r->index) ? p.src(r) : r->operandAt(0).get())->index, st.stream);
         hoisted(ch.rots, ch.ell);
         check(evab_rotate_modup_many(c, ch.ell, (int)elts.size(), A + ch.outOff, out, A + p.hoistExtOff[ch.gid], elts.data(), keys.data(), cadds.data(), work, stream));
         return;
@@ -475,10 +479,11 @@ private:
         if (*t.rotation == 0) check(evab_copy(c, o.ell, out, P(0), 2, stream));  // rotate_vector(0): copy
         else {
           const u64 elt = galoisElt(t);
+          const u64 *in = A + p.vals[p.src(&t)->index].off;   // a composed rotation's last hop reads the hop before it
           if (st.hoist >= 0 && p.opt.hoistModUp)
-            check(evab_rotate_modup_prepared(c, o.ell, out, P(0), A + p.hoistExtOff[st.hoist], elt, galoisKey(elt), hoistConst(elt, o.ell), work, stream));
-          else if (st.hoist >= 0) check(evab_rotate_prepared(c, o.ell, out, P(0), A + p.hoistOff[st.hoist], elt, galoisKey(elt), work, stream));
-          else check(evab_rotate(c, o.ell, out, P(0), elt, galoisKey(elt), work, stream));
+            check(evab_rotate_modup_prepared(c, o.ell, out, in, A + p.hoistExtOff[st.hoist], elt, galoisKey(elt), hoistConst(elt, o.ell), work, stream));
+          else if (st.hoist >= 0) check(evab_rotate_prepared(c, o.ell, out, in, A + p.hoistOff[st.hoist], elt, galoisKey(elt), work, stream));
+          else check(evab_rotate(c, o.ell, out, in, elt, galoisKey(elt), work, stream));
         }
         break;
       case Op::Relinearize: check(evab_relinearize(c, o.ell, out, P(0), relinKey(), work, stream)); break;

@@ -3,6 +3,7 @@
 // the arena layout.  Pure host code: no device calls, so that plans can be built and checked without a GPU
 // (tests/test_planner.py).  executor.hpp materialises a Plan on the device and replays it.
 #pragma once
+#include "../host_tables.hpp"
 #include "arena_packer.hpp"
 #include "ir.hpp"
 #include <algorithm>
@@ -123,13 +124,23 @@ struct WorkSizes {
 struct Plan {
   ExecOptions opt;
   std::uint64_t N = 0;
-  std::vector<Term *> order;                    // the program's terms in topological order
+  std::uint64_t terms = 0;                      // term indices: the program's terms, then the plan's own rotation hops
+  std::vector<Term *> order;                    // the program's terms (and hops) in topological order
   std::vector<Term *> byIndex;                  // term index -> term
   std::vector<std::uint64_t> canon;             // term index -> index of the first identical term (itself when unique)
   std::vector<ValueInfo> vals;
   std::vector<std::vector<double>> constants;   // term index -> the expanded vector of a Constant term (empty otherwise)
   std::vector<char> dyn;                        // term index -> depends on a raw input
   std::size_t cipherOps = 0;
+  // composeRotations: rotations whose step has no Galois key run as chains of rotations by NAF terms.  The intermediate hops are
+  // terms of the plan (RotateLeftConst by the term's signed step, no operands, indices from the program's termCount()); their
+  // storage is a program of their own, never the user's
+  std::unique_ptr<Program> hopProgram;
+  std::vector<Term::Ptr> hops;
+  std::unordered_map<std::uint64_t, const Term *> chainSrc;   // hop or composed rotation -> the ciphertext it rotates
+  std::unordered_map<std::uint64_t, int> lastHop;             // composed rotation of the program -> the step of its last hop
+  std::map<std::uint64_t, std::vector<int>> chain;            // every key-switched rotation of the program -> the steps it applies
+  long composedRotations = 0;
   std::vector<const Term *> hoistSrc;           // hoist group -> the ciphertext its rotations read
   std::vector<std::size_t> hoistOff, hoistExtOff;   // arena word offsets of every hoist buffer and of its extended digits (hoistModUp)
   std::vector<char> needsC0;                    // hoist group feeds evab_rotate_modup_many / evab_lazy_rotsum
@@ -162,6 +173,13 @@ struct Plan {
   // canonical (first) occurrence of a term that repeats an earlier one (dedupTerms)
   const Term *C(const Term *t) const { return byIndex[canon[t->index]]; }
   std::uint64_t aliasSource(const Term *t) const { return canon[t->index] != t->index ? canon[t->index] : t->operandAt(0)->index; }
+  // the ciphertext a rotation reads: its operand, or the previous hop of its chain
+  const Term *src(const Term *r) const { auto f = chainSrc.find(r->index); return f != chainSrc.end() ? f->second : C(r->operandAt(0).get()); }
+  // the step a rotation applies (SEAL's rotate_vector argument): its own, or the last hop's of its chain
+  int stepOf(const Term *r) const {
+    if (auto f = lastHop.find(r->index); f != lastHop.end()) return f->second;
+    return r->op == Op::RotateLeftConst ? *r->rotation : -*r->rotation;
+  }
   // every rotation the plan issues, and whether it uses a shared mod-up (and so the hoist constant of its (element, ell))
   template <class F> void forEachRotation(F f) const {
     for (auto &st : steps)
@@ -188,6 +206,7 @@ struct Plan {
     long elided = 0;
     for (auto &t : order) if ((t->op == Op::RotateLeftConst || t->op == Op::RotateRightConst) && vals[t->index].fused) elided++;
     m["elided_rotations"] = elided;
+    m["composed_rotations"] = composedRotations; m["composed_hops"] = (long)hops.size();
     m["arena_bytes"] = (long)arenaBytes(); m["arena_bytes_unpacked"] = (long)unpackedBytes; m["packed"] = packed ? 1 : 0;
     m["reuse_waits"] = reuseWaits;
     long constWords = 0;   // plaintexts of plan-time constants, resident for the plan's lifetime
@@ -201,12 +220,15 @@ struct Plan {
 // The passes, run in this order by buildPlan (below).  Each reads what the earlier ones derived.
 class Planner {
 public:
-  Planner(Program &prog, const ExecOptions &opt, std::uint64_t N, int k, const WorkSizes &ws) : prog_(prog), ws_(ws), k_(k) {
+  // galoisElements: the Galois elements that have keys (null: every step has its own)
+  Planner(Program &prog, const ExecOptions &opt, std::uint64_t N, int k, const WorkSizes &ws, const std::set<std::uint64_t> *galoisElements)
+      : prog_(prog), ws_(ws), k_(k), elts_(galoisElements) {
     p.opt = opt;
     p.N = N;
   }
   Plan run(std::size_t arenaLimit) {
     inferValues();
+    composeRotations();
     fuseSums();
     groupRotations();
     sumRotations();
@@ -222,7 +244,7 @@ private:
   void inferValues() {
     const ExecOptions &opt = p.opt;
     for (auto &t : prog_.toposort()) p.order.push_back(t.get());  // raw: the plan lives inside the Program (attachment)
-    const std::uint64_t TC = prog_.termCount();
+    const std::uint64_t TC = p.terms = prog_.termCount();
     p.vals.assign(TC, ValueInfo{});
     if (opt.batch < 1) throw std::invalid_argument("batch must be >= 1");
     p.constants.assign(TC, {});
@@ -317,6 +339,73 @@ private:
     }
   }
 
+  // ---- 1b. composed rotations (SEAL 3.6 Evaluator::rotate_internal): a ciphertext rotation whose step has no Galois key is the chain
+  // of rotations by the NAF terms of its step (evab_host::rotation_hops), each an ordinary key switch.  The chains of one source
+  // share their prefixes, a trie keyed by Galois elements.  A prefix node is a plan-owned hop, or the value of a program rotation
+  // of the same source that computes exactly it: a rotation by its single term, or a keyless rotation whose own chain it is (a
+  // longer prefix whose sum has a key of its own is a different value).  The last hop of a chain is the program's term itself.
+  // Later passes see ordinary rotations: Plan::src and Plan::stepOf give what each reads and applies.  Without composed rotations
+  // the plan is unchanged.
+  void composeRotations() {
+    const std::uint64_t N = p.N;
+    auto has = [&](std::uint64_t e) { return !elts_ || elts_->count(e) > 0; };
+    std::vector<Term *> rots;
+    for (Term *t : p.order)
+      if ((t->op == Op::RotateLeftConst || t->op == Op::RotateRightConst) && *t->rotation != 0 && p.vals[t->index].kind == Kind::Cipher &&
+          p.canon[t->index] == t->index && evab_host::galois_elt_from_step(N, p.stepOf(t)))   // (a step too large: the executor's error)
+        rots.push_back(t);
+    // (source, Galois elements of the chain) -> the term holding that value; program rotations first, in program order
+    std::map<std::pair<std::uint64_t, std::vector<std::uint64_t>>, const Term *> node;
+    auto eltsOf = [&](const std::vector<int> &steps, std::size_t n) {
+      std::vector<std::uint64_t> e;
+      for (std::size_t j = 0; j < n; j++) e.push_back(evab_host::galois_elt_from_step(N, steps[j]));
+      return e;
+    };
+    for (Term *t : rots) {
+      std::vector<int> &hops = p.chain[t->index] = evab_host::rotation_hops(N, p.stepOf(t), has);
+      node.emplace(std::make_pair(p.src(t)->index, eltsOf(hops, hops.size())), t);
+    }
+    for (Term *t : rots) {
+      const int s = p.stepOf(t);
+      const std::vector<int> hops = p.chain.at(t->index);
+      if (has(evab_host::galois_elt_from_step(N, s))) continue;
+      const Term *prev = p.src(t);
+      const std::uint64_t x = prev->index;
+      for (std::size_t j = 1; j < hops.size(); j++) {
+        auto key = std::make_pair(x, eltsOf(hops, j));
+        auto f = node.find(key);
+        if (f == node.end()) {   // a plan-owned hop
+          if (!p.hopProgram) p.hopProgram = std::make_unique<Program>("rotation hops", prog_.getVecSize());
+          Term::Ptr h = p.hopProgram->makeTerm(Op::RotateLeftConst);
+          h->rotation = hops[j - 1];
+          h->index = p.terms++;
+          ValueInfo v = p.vals[t->index];
+          v.alias = v.fused = false;
+          p.vals.push_back(v); p.canon.push_back(h->index); p.byIndex.push_back(h.get()); p.constants.emplace_back();
+          p.chainSrc[h->index] = prev;
+          p.hops.push_back(h);
+          f = node.emplace(std::move(key), h.get()).first;
+        }
+        prev = f->second;
+      }
+      p.chainSrc[t->index] = prev;
+      p.lastHop[t->index] = hops.back();
+      p.composedRotations++;
+    }
+    if (!p.composedRotations) return;
+    // every hop and every prefix value before its first reader (the sources of the chains come before them already)
+    std::vector<Term *> order;
+    std::vector<char> placed(p.terms, 0);
+    std::function<void(Term *)> place = [&](Term *t) {
+      if (placed[t->index]) return;
+      placed[t->index] = 1;
+      if (auto f = p.chainSrc.find(t->index); f != p.chainSrc.end()) place(p.byIndex[f->second->index]);
+      order.push_back(t);
+    };
+    for (Term *t : p.order) place(t);
+    p.order = std::move(order);
+  }
+
   // ---- 2. fused sums: a tree of cipher+cipher Adds whose inner nodes have a single use collapses into
   // one kernel; leaves that are single-use multiply_plain results are multiplied on the fly
   // (Sobel / Harris filter taps: sum_i rot_i(x) * w_i).  Same canonical result, see evab_sum_terms.
@@ -378,11 +467,11 @@ private:
     for (auto &t : p.order)
       if ((t->op == Op::RotateLeftConst || t->op == Op::RotateRightConst) && *t->rotation != 0 && p.vals[t->index].kind == Kind::Cipher &&
           p.vals[t->index].ell <= 15 && !p.vals[t->index].alias)
-        bySrc[p.canon[t->operandAt(0)->index]].push_back(t);
+        bySrc[p.src(t)->index].push_back(t);
     for (auto &kv : bySrc) {
       if (kv.second.size() < 2) continue;
       const int gid = (int)p.hoistSrc.size();
-      p.hoistSrc.push_back(p.C(kv.second.front()->operandAt(0).get()));
+      p.hoistSrc.push_back(p.src(kv.second.front()));
       for (const Term *r : kv.second) hoistOf_[r->index] = gid;
     }
     if (p.opt.hoistModUp) p.numFlags = p.hoistSrc.size();   // one zero-coefficient flag per group
@@ -399,9 +488,11 @@ private:
     const ExecOptions &opt = p.opt;
     const bool exactSums = !opt.approxHoist && opt.rotationSums;
     if (!((opt.approxHoist || exactSums) && opt.hoistModUp && opt.fuseSums)) return;
-    const std::uint64_t TC = prog_.termCount();
+    const std::uint64_t TC = p.terms;
     std::vector<int> usesAll = useCounts(), lazyUses(TC, 0), wsumLeaves(TC, 0), pos(TC, 0);
     for (std::size_t i = 0; i < p.order.size(); i++) pos[p.order[i]->index] = (int)i;
+    std::set<const Term *> chainRead;   // rotations that a hop of a composed rotation reads
+    for (auto &kv : p.chainSrc) chainRead.insert(kv.second);
     auto scalarWeight = [&](const Term *pt, double &v) {
       if (pt->op != Op::Encode || pt->operandAt(0)->op != Op::Constant || !replicatedScalar(pt)) return false;
       v = p.constants[pt->operandAt(0)->index][0];
@@ -425,6 +516,7 @@ private:
       for (int i = 0; i < (int)leaves.size(); i++) {
         if (kinds[i] != 1 || !rotLeaf(leaves[i])) continue;
         if (exactSums && wsumLeaves[leaves[i].first->index] != usesAll[leaves[i].first->index]) continue;
+        if (chainRead.count(leaves[i].first)) continue;   // materialised for the hops that read it: used as it is
         byGroup[hoistOf_.at(leaves[i].first->index)].push_back(i);
       }
       auto isZero = [&](int i) { double v = 1.0; return exactSums && scalarWeight(leaves[i].second, v) && v == 0.0; };
@@ -433,8 +525,10 @@ private:
       for (auto &kv : byGroup)
         for (std::size_t b = 0; b < kv.second.size(); b += 16)
           slices.emplace_back(kv.first, std::vector<int>(kv.second.begin() + b, kv.second.begin() + std::min(kv.second.size(), b + 16)));
+      std::vector<int> zeroSlices;   // leaves of slices whose weights are all 0.0: dropped when the sum takes a rotation sum call
       for (auto &kv : slices) {
-        if (kv.second.size() < 2 || std::all_of(kv.second.begin(), kv.second.end(), isZero)) continue;
+        if (std::all_of(kv.second.begin(), kv.second.end(), isZero)) { zeroSlices.insert(zeroSlices.end(), kv.second.begin(), kv.second.end()); continue; }
+        if (kv.second.size() < 2) continue;
         // sums over rotations of the same ciphertext share one call (and the inner products of the rotations they have in
         // common), as long as the later sum's weights are available when the first one runs
         int li = -1;
@@ -474,6 +568,7 @@ private:
         p.lazyOfRoot[t->index].emplace_back(li, (int)L.roots.size() - 1);
       }
       if (!p.lazyOfRoot.count(t->index)) continue;
+      for (int i : zeroSlices) { drop[i] = 1; lazyUses[leaves[i].first->index]++; }
       if (exactSums) {   // the other scalar-weighted leaves: taps of the first call, when they are computed before that call is issued
         const auto [li, o] = p.lazyOfRoot.at(t->index).front();
         LazySum &L = p.lazy[li];
@@ -533,7 +628,7 @@ private:
   // Static groups (constants only) are encoded once per plan when cacheConstants is
   // set, otherwise every run like the reference (seal_executor.h:303-308).
   void groupEncodes() {
-    p.dyn.assign(prog_.termCount(), 0);
+    p.dyn.assign(p.terms, 0);
     for (auto &t : p.order) {
       bool d = (t->op == Op::Input && p.vals[t->index].kind == Kind::Raw);
       for (auto &o : t->getOperands()) d = d || p.dyn[o->index];
@@ -576,7 +671,7 @@ private:
   // ---- 7. stream assignment + event edges.  Producers are identified by term index, or termCount + hoist group,
   // + rotation sum, + chunk for the pseudo steps.
   void schedule() {
-    const std::uint64_t TC = prog_.termCount(), H = p.hoistSrc.size(), L = p.lazy.size();
+    const std::uint64_t TC = p.terms, H = p.hoistSrc.size(), L = p.lazy.size();
     const int S = std::max(1, p.opt.numStreams);
     const std::size_t NP = TC + H + L + p.chunks.size();
     std::unordered_map<std::uint64_t, std::uint64_t> prodOf;   // rotation term -> the chunk step that produces it
@@ -675,8 +770,10 @@ private:
         forced = g.stream;
       }
       std::size_t w = 0;
-      if (t->op == Op::Relinearize || ((t->op == Op::RotateLeftConst || t->op == Op::RotateRightConst) && *t->rotation != 0))
+      if (t->op == Op::Relinearize)
         w = ws_.keyswitch(p.vals[t->operandAt(0)->index].ell) / 8;
+      else if ((t->op == Op::RotateLeftConst || t->op == Op::RotateRightConst) && *t->rotation != 0)
+        w = ws_.keyswitch(p.vals[p.src(t)->index].ell) / 8;
       else if (t->op == Op::Rescale)
         w = ws_.rescale(p.vals[t->operandAt(0)->index].size) / 8;
       if (auto h = hoistOf_.find(t->index); h != hoistOf_.end()) {   // the group's shared inverse NTT goes first
@@ -713,7 +810,7 @@ private:
   // Regions in layout order: values (those later absorbed into a fused sum, a chunk or a rotation sum output keep their words in
   // the one-offset-per-value layout, unwritten), hoist groups, rotation sums, chunks, encode groups, flags, workspaces
   void regionTable() {
-    const std::uint64_t TC = prog_.termCount(), H = p.hoistSrc.size(), L = p.lazy.size();
+    const std::uint64_t TC = p.terms, H = p.hoistSrc.size(), L = p.lazy.size();
     std::unordered_map<std::uint64_t, int> stepOf;   // producer -> step
     for (int i = 0; i < (int)p.steps.size(); i++) stepOf[p.steps[i].producer] = i;
     auto writerOf = [&](std::uint64_t producer) { auto f = stepOf.find(producer); return f == stepOf.end() ? -1 : f->second; };
@@ -841,9 +938,16 @@ private:
 
   // uses of every canonical term by canonical terms
   std::vector<int> useCounts() const {
-    std::vector<int> uses(prog_.termCount(), 0);
-    for (auto &t : p.order) if (p.canon[t->index] == t->index) for (auto &o : t->getOperands()) uses[p.canon[o->index]]++;
+    std::vector<int> uses(p.terms, 0);
+    for (auto &t : p.order) if (p.canon[t->index] == t->index) for (const Term *o : operands(t)) uses[o->index]++;
     return uses;
+  }
+  // the canonical terms a term reads (a rotation of a chain: the previous hop)
+  std::vector<const Term *> operands(const Term *t) const {
+    if (auto f = p.chainSrc.find(t->index); f != p.chainSrc.end()) return {f->second};
+    std::vector<const Term *> ops;
+    for (auto &o : t->getOperands()) ops.push_back(p.C(o.get()));
+    return ops;
   }
   // the Encode term's vector is a replicated scalar (the uniform encoder's predicate)
   bool replicatedScalar(const Term *enc) const {
@@ -854,7 +958,7 @@ private:
   std::vector<const Term *> stepOperands(const Term *t) const {
     std::vector<const Term *> ops;
     auto f = sumOf_.find(t->index);
-    if (f == sumOf_.end()) { for (auto &o : t->getOperands()) ops.push_back(p.C(o.get())); return ops; }
+    if (f == sumOf_.end()) return operands(t);
     for (auto &l : f->second) { ops.push_back(l.first); if (l.second) ops.push_back(l.second); }
     return ops;
   }
@@ -868,6 +972,7 @@ private:
   Program &prog_;
   const WorkSizes &ws_;
   int k_;
+  const std::set<std::uint64_t> *elts_;
   Plan p;
   std::vector<Term *> encodeTerms_;
   std::unordered_map<std::uint64_t, std::vector<std::pair<const Term *, const Term *>>> sumOf_;   // fused sum -> leaves
@@ -879,8 +984,10 @@ private:
 };
 
 // N, k: the ring degree and the modulus count (with the key-switch prime); arenaLimit: bytes the arena may take
-inline Plan buildPlan(Program &program, const ExecOptions &opt, std::uint64_t N, int k, std::size_t arenaLimit, const WorkSizes &ws) {
-  return Planner(program, opt, N, k, ws).run(arenaLimit);
+// galoisElements: the Galois elements that have keys; rotations by other steps are composed (null: every step has its own key)
+inline Plan buildPlan(Program &program, const ExecOptions &opt, std::uint64_t N, int k, std::size_t arenaLimit, const WorkSizes &ws,
+                      const std::set<std::uint64_t> *galoisElements = nullptr) {
+  return Planner(program, opt, N, k, ws, galoisElements).run(arenaLimit);
 }
 
 }  // namespace evab

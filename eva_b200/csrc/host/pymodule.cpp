@@ -199,7 +199,10 @@ PYBIND11_MODULE(_eva_b200, m) {
   py::class_<ExecOptions> planOptions(m, "_PlanOptions");
   planOptions.def(py::init<>());
   defSetOptions(planOptions);
-  m.def("_plan", [](Program &prog, std::uint64_t N, int k, const py::dict &options, int batch) {
+  // galois_elements: the elements that have keys (None: every step has its own).  Besides the plan's shape it returns "chains" (every
+  // key-switched rotation of the program -> the steps it applies, composeRotations), "sources" (hops and composed rotations -> the
+  // term each reads) and "rotations" (every rotation the plan issues: (term, the term it reads, step))
+  m.def("_plan", [](Program &prog, std::uint64_t N, int k, const py::dict &options, int batch, std::optional<std::set<u64>> galoisElements) {
     py::object holder = py::cast(ExecOptions{});
     holder.attr("set_options")(**options);
     ExecOptions opt = holder.cast<ExecOptions>();
@@ -211,7 +214,7 @@ PYBIND11_MODULE(_eva_b200, m) {
     ws.rotateWsum = [N](int ell, int n, int nout) { return (std::size_t)(n + nout) * (ell + 1) * N * 8; };
     ws.lazyRotsum = [N](int ell, int nout) { return (std::size_t)nout * (ell + 1) * N * 8; };
     ws.encode = [N](int count) { return (std::size_t)count * N * 16; };
-    const Plan p = buildPlan(prog, opt, N, k, opt.arenaLimit ? opt.arenaLimit : SIZE_MAX, ws);
+    const Plan p = buildPlan(prog, opt, N, k, opt.arenaLimit ? opt.arenaLimit : SIZE_MAX, ws, galoisElements ? &*galoisElements : nullptr);
     static const char *kinds[] = {"Term", "Hoist", "RotationChunk", "RotationSum"};
     py::list steps, regions;
     for (auto &st : p.steps) steps.append(py::make_tuple(kinds[(int)st.kind], st.term->index, st.stream, st.waits, st.record));
@@ -223,10 +226,16 @@ PYBIND11_MODULE(_eva_b200, m) {
         const std::size_t rows = v.kind == Kind::Cipher ? (std::size_t)v.size * v.ell : v.ell + (t->op == Op::Encode && p.groups[p.groupIndex.at(t->index)].withP);
         values[py::int_(t->index)] = py::make_tuple(v.off, rows * N, r);
       }
-    py::dict d;
+    py::dict d, sources;
+    py::list rotations;
+    for (auto &kv : p.chainSrc) sources[py::int_(kv.first)] = kv.second->index;
+    p.forEachRotation([&](const Term *r, bool) { rotations.append(py::make_tuple(r->index, p.src(r)->index, p.stepOf(r))); });
     d["steps"] = steps; d["regions"] = regions; d["values"] = values; d["stride"] = p.stride; d["stats"] = p.planStats();
+    d["chains"] = p.chain; d["sources"] = sources; d["rotations"] = rotations;
     return d;
-  }, py::arg("program"), py::arg("N"), py::arg("k"), py::arg("options") = py::dict(), py::arg("batch") = 1);
+  }, py::arg("program"), py::arg("N"), py::arg("k"), py::arg("options") = py::dict(), py::arg("batch") = 1, py::arg("galois_elements") = py::none());
+  // test hook: the steps that get a Galois key under generate_keys / B200Server(rotation_keys=...)
+  m.def("_rotation_key_steps", &rotationKeySteps, py::arg("params"), py::arg("rotation_keys"));
   m.def("set_num_threads", [](int) {}, py::arg("num_threads"),
         "Kept for API compatibility: the DAG is scheduled on CUDA streams, not CPU threads.");
   py::class_<int>(m, "_GaloisGuard").def(py::init());
@@ -496,12 +505,14 @@ PYBIND11_MODULE(_eva_b200, m) {
   py::class_<B200Server> srv(mb, "B200Server",
                              "Executes compiled programs for many clients: each client's evaluation keys are a tenant of a key bank of fixed "
                              "capacity, the plans are shared by all tenants, and every instance of a batch runs with its own tenant's keys");
-  srv.def(py::init([](const CKKSParameters &params, int capacity, int device, std::optional<int> maxTenants) {
-        return std::make_unique<B200Server>(params, capacity, device, maxTenants ? *maxTenants : -1);
-      }), py::arg("params"), py::arg("capacity") = 64, py::arg("device") = 0, py::arg("max_tenants") = py::none(),
+  srv.def(py::init([](const CKKSParameters &params, int capacity, int device, std::optional<int> maxTenants, const std::string &rotationKeys) {
+        return std::make_unique<B200Server>(params, capacity, device, maxTenants ? *maxTenants : -1, rotationKeys);
+      }), py::arg("params"), py::arg("capacity") = 64, py::arg("device") = 0, py::arg("max_tenants") = py::none(), py::arg("rotation_keys") = "program",
       "capacity: device slots (key-bank regions).  max_tenants None or == capacity: a tenant id is its slot, filled when its keys are "
       "added.  max_tenants > capacity: up to max_tenants tenants' keys in page-locked host memory, paged into the slots (least "
-      "recently used first) as batches need them")
+      "recently used first) as batches need them.  rotation_keys: the Galois keys every tenant supplies -- \"program\", one per "
+      "rotation step of the program; \"power_of_two\", one per NAF term of its steps (the other rotations are composed from them, "
+      "as SEAL's rotate_vector does)")
       .def("add_raw_keys", [](B200Server &s, const u64arr &relin, const std::map<u64, u64arr> &galois) {
         const std::size_t kk = s.shared()->dev->k(), N = s.shared()->dev->N();
         requireShape(relin, {kk - 1, 2, kk, N}, "relinearization key");
@@ -616,8 +627,10 @@ PYBIND11_MODULE(_eva_b200, m) {
         d["compressed_tenants"] = pg ? pg->compressedTenants() : b.compressedTenants();
         d["fills"] = b.fills();
         d["evictions"] = pg ? pg->cache().evictions() : 0;
+        d["rotation_keys"] = s.rotationKeys();
         return d;
-      }, "capacity / device_slots: key-bank regions; max_tenants: tenant ids (more than the slots: paging); resident: the tenants "
+      }, "capacity / device_slots: key-bank regions; rotation_keys: the key set of galois_elements (\"program\" or \"power_of_two\"); "
+         "max_tenants: tenant ids (more than the slots: paging); resident: the tenants "
          "holding a slot; host_key_bytes: page-locked host memory of the paged keys (compressed tenants: c0 rows and seeds); "
          "compressed_tenants: tenants added in compressed form; fills: slots filled (keys uploaded and "
          "constants computed); evictions: resident tenants displaced by a fill")
@@ -635,8 +648,11 @@ PYBIND11_MODULE(_eva_b200, m) {
            py::arg("program"), py::arg("index"), py::arg("batch") = 1, py::arg("instance") = 0);
   defSetOptions(srv);
 
-  mb.def("generate_keys", [](const CKKSParameters &p, int device, std::uint64_t seed) { return generateKeys(p, device, seed); },
-         py::arg("abstract_params"), py::arg("device") = 0, py::arg("seed") = 0);
+  mb.def("generate_keys", [](const CKKSParameters &p, int device, std::uint64_t seed, const std::string &rotationKeys) {
+           return generateKeys(p, device, seed, rotationKeys);
+         }, py::arg("abstract_params"), py::arg("device") = 0, py::arg("seed") = 0, py::arg("rotation_keys") = "program",
+         "rotation_keys: \"program\" -- a Galois key for every rotation step of the program; \"power_of_two\" -- one for every NAF term "
+         "of its nonzero steps (but +-N/2), ascending, from which every rotation of the program is composed as SEAL's rotate_vector does");
   // test/benchmark hook: evaluation context from externally supplied key material
   mb.def("context_from_raw_keys", [](std::uint64_t N, const std::vector<u64> &primes, const u64arr &relin, const std::map<u64, u64arr> &galois, int device) {
     auto s = std::make_shared<Shared>();

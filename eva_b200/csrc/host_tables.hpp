@@ -5,6 +5,8 @@
 #pragma once
 #include "modarith.cuh"
 #include <cmath>
+#include <stdexcept>
+#include <string>
 #include <vector>
 
 namespace evab_host {
@@ -134,6 +136,42 @@ inline u64 galois_elt_from_step(u64 N, int steps) {
   u64 s = steps < 0 ? N / 2 - pos : pos, g = 1;
   for (u64 i = 0; i < s; i++) g = (g * 3) & (m - 1);
   return g;
+}
+// SEAL's util::naf: `value` as signed powers of two, no two of them adjacent, lowest first
+inline std::vector<int> naf(int value) {
+  std::vector<int> res;
+  const bool neg = value < 0;
+  long long v = neg ? -(long long)value : value;
+  for (int i = 0; v; i++) {
+    const long long z = (v & 1) ? 2 - (v & 3) : 0;
+    v = (v - z) >> 1;
+    if (z) res.push_back((int)((neg ? -z : z) << i));
+  }
+  return res;
+}
+// The NAF terms of a rotation by `steps` that Evaluator::rotate_internal applies when `steps` has no Galois key of its own: every
+// term of naf(steps) in order, but those of magnitude N/2 (no rotation of the N/2 slots)
+inline std::vector<int> naf_rotation_terms(u64 N, int steps) {
+  std::vector<int> out;
+  for (int t : naf(steps)) if ((u64)(t < 0 ? -(long long)t : t) != N / 2) out.push_back(t);
+  return out;
+}
+// The rotations that SEAL 3.6's rotate_vector(steps) applies, one key switch each, when the Galois keys present are the elements
+// for which hasKey is true: {steps} when its own element has a key, else naf_rotation_terms(N, steps), each of which must have a
+// key.  A missing key throws std::invalid_argument naming steps, the term and its element.  steps != 0, |steps| < N/2.
+template <class HasKey>
+std::vector<int> rotation_hops(u64 N, int steps, HasKey hasKey) {
+  const u64 elt = galois_elt_from_step(N, steps);
+  if (!elt) throw std::invalid_argument("step count too large");
+  if (hasKey(elt)) return {steps};
+  std::vector<int> hops = naf_rotation_terms(N, steps);
+  for (int t : hops) {
+    const u64 e = galois_elt_from_step(N, t);
+    if (!hasKey(e))
+      throw std::invalid_argument("Galois key not present: the rotation by " + std::to_string(steps) + " steps is composed of NAF terms, and the term " +
+                                  std::to_string(t) + " (Galois element " + std::to_string(e) + ") has no key");
+  }
+  return hops;
 }
 inline void galois_table(u64 N, int logN, u64 elt, std::vector<u32> &tab) {
   tab.resize(N);
