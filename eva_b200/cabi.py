@@ -48,6 +48,8 @@ _SIGS = {
     "evab_hoist_const_levels_bytes": (szt, [vp]),
     "evab_rotate_hoist_const_levels_work_bytes": (szt, [vp, ci]),
     "evab_rotate_hoist_const_levels": (ci, [vp, ci, u64p, vp, vp, vp, vp]),
+    "evab_hoist_indicators_bytes": (szt, [vp, ci]),
+    "evab_hoist_indicators": (ci, [vp, ci, u64p, vp, vp]),
     "evab_expand_key_uniform": (ci, [vp, ci, vp, u64p, vp, vp]),
     "evab_expand_cipher_uniform": (ci, [vp, ci, vp, vp, vp, u64p, vp]),
     "evab_rotate_modup_prepared": (ci, [vp, ci, vp, vp, vp, u64, vp, vp, vp, vp]),
@@ -87,6 +89,7 @@ _SIGS = {
     "evab_copy": (ci, [vp, ci, vp, vp, ci, vp]),
     "evab_set_batch": (ci, [ci, szt, szt]),
     "evab_set_key_bank": (ci, [vp, szt]),
+    "evab_set_hoist_inline": (ci, [ci]),
     "evab_mod_switch": (ci, [vp, ci, vp, vp, ci, vp]),
     "evab_keyswitch_work_bytes": (szt, [vp, ci]),
     "evab_relinearize": (ci, [vp, ci, vp, vp, vp, vp, vp]),

@@ -66,6 +66,12 @@ extern "C" int evab_set_key_bank(const int32_t *d_tenant_of_instance, size_t ten
   g_bank.stride = d_tenant_of_instance ? (long long)tenant_stride_words : 0;
   return 0;
 }
+// thread-local inline hoist constants (evab_set_hoist_inline): the cadd operands of the hoisted rotations are indicator rows
+static thread_local bool g_inline = false;
+extern "C" int evab_set_hoist_inline(int on) {
+  g_inline = on != 0;
+  return 0;
+}
 
 
 // ---------------------------------------------------------------------------
@@ -208,25 +214,27 @@ __global__ void __launch_bounds__(256) k_sum_terms(const SumArgs A, const long l
 }
 // key offset of this block's instance: BANK = false is the shared-key launch (offset 0, the table is not read)
 template <bool BANK> __device__ __forceinline__ long long key_off(const KeyBankSel &K) { return BANK ? (long long)__ldg(K.tenant + blockIdx.z) * K.stride : 0; }
-template <bool BANK> __global__ void __launch_bounds__(256) k_ks_inner(const IpArgs A, const long long bstride, const KeyBankSel K) {
+// INL: inline hoist constants (ks_inner_elem)
+template <bool BANK, bool INL> __global__ void __launch_bounds__(256) k_ks_inner(const IpArgs A, const long long bstride, const KeyBankSel K) {
   const long long off = (long long)blockIdx.z * bstride;   // parameters stay in constant memory: no local copy
   const long long koff = key_off<BANK>(K);
   for (int j = (blockIdx.x * blockDim.x + threadIdx.x) * 2; j < A.N; j += gridDim.x * blockDim.x * 2)
-    ks_inner_elem(A, blockIdx.y, j, off, koff);
+    ks_inner_elem<INL>(A, blockIdx.y, j, off, koff);
 }
 __global__ void __launch_bounds__(256) k_scale_c0(const u64 *c0, u64 *ext, const PrimeDev *primes, int ell, int k, int N, const long long bstride) {
   const long long off = (long long)blockIdx.z * bstride;
   for (int j = blockIdx.x * blockDim.x + threadIdx.x; j < N; j += gridDim.x * blockDim.x) scale_c0_elem(c0, ext, primes, ell, k, N, blockIdx.y, j, off);
 }
-template <bool BANK> __global__ void __launch_bounds__(256, 4) k_rot_many(const RotManyArgs A, const long long bstride, const KeyBankSel K) {
+// INL: 3 blocks per SM (80 registers) -- at 4 the inline instance spills about 100 bytes
+template <bool BANK, bool INL> __global__ void __launch_bounds__(256, INL ? 3 : 4) k_rot_many(const RotManyArgs A, const long long bstride, const KeyBankSel K) {
   const long long off = (long long)blockIdx.z * bstride, koff = key_off<BANK>(K);
   const int i = blockIdx.y / (A.ell + 1), mi = blockIdx.y % (A.ell + 1);
-  for (int j = (blockIdx.x * blockDim.x + threadIdx.x) * 2; j < A.N; j += gridDim.x * blockDim.x * 2) rot_many_elem(A, i, mi, j, off, koff);
+  for (int j = (blockIdx.x * blockDim.x + threadIdx.x) * 2; j < A.N; j += gridDim.x * blockDim.x * 2) rot_many_elem<INL>(A, i, mi, j, off, koff);
 }
 // grid.y = row of the extended basis; every thread loops over the rotations, so blocks are kept small for more of them
-template <int NOUT, bool BANK> __global__ void __launch_bounds__(128) k_rot_wsum_ip(const WsumIpArgs A, const long long bstride, const KeyBankSel K) {
+template <int NOUT, bool BANK, bool INL> __global__ void __launch_bounds__(128) k_rot_wsum_ip(const WsumIpArgs A, const long long bstride, const KeyBankSel K) {
   const long long off = (long long)blockIdx.z * bstride, koff = key_off<BANK>(K);
-  for (int j = (blockIdx.x * blockDim.x + threadIdx.x) * 2; j < A.N; j += gridDim.x * blockDim.x * 2) rot_wsum_ip_elem<NOUT>(A, blockIdx.y, j, off, koff);
+  for (int j = (blockIdx.x * blockDim.x + threadIdx.x) * 2; j < A.N; j += gridDim.x * blockDim.x * 2) rot_wsum_ip_elem<NOUT, INL>(A, blockIdx.y, j, off, koff);
 }
 // grid.y = (polynomial, residue) of the outputs
 __global__ void __launch_bounds__(256) k_rot_wsum(const WsumArgs A, const long long bstride) {
@@ -411,6 +419,7 @@ struct CudaBE {
   const evab_ctx *c;
   cudaStream_t st;
   int error(const char *m) { return fail(m); }
+  bool hoist_inline() const { return g_inline; }
   void count(unsigned n = 1) const { c->launches.fetch_add(n, std::memory_order_relaxed); }
   dim3 grid(int rows, int per_thread = 2) const {
     int per_row = (int)(c->v.N / per_thread / 256);
@@ -471,8 +480,11 @@ struct CudaBE {
   }
   int inner(const IpArgs &A) {
     count();
-    if (g_bank.tenant) k_ks_inner<true><<<grid(A.ell + 1), 256, 0, st>>>(A, g_batch.stride, g_bank);
-    else k_ks_inner<false><<<grid(A.ell + 1), 256, 0, st>>>(A, g_batch.stride, g_bank);
+    const dim3 g = grid(A.ell + 1);
+    const bool inl = g_inline && A.cadd;   // only the hoisted form has a constant to form
+    if (g_bank.tenant) { if (inl) k_ks_inner<true, true><<<g, 256, 0, st>>>(A, g_batch.stride, g_bank); else k_ks_inner<true, false><<<g, 256, 0, st>>>(A, g_batch.stride, g_bank); }
+    else if (inl) k_ks_inner<false, true><<<g, 256, 0, st>>>(A, g_batch.stride, g_bank);
+    else k_ks_inner<false, false><<<g, 256, 0, st>>>(A, g_batch.stride, g_bank);
     CUDA_OK(cudaGetLastError());
     return 0;
   }
@@ -484,24 +496,27 @@ struct CudaBE {
   }
   int rot_many(const RotManyArgs &A) {
     count();
-    if (g_bank.tenant) k_rot_many<true><<<grid(A.n * (A.ell + 1)), 256, 0, st>>>(A, g_batch.stride, g_bank);
-    else k_rot_many<false><<<grid(A.n * (A.ell + 1)), 256, 0, st>>>(A, g_batch.stride, g_bank);
+    const dim3 g = grid(A.n * (A.ell + 1));
+    if (g_bank.tenant) { if (g_inline) k_rot_many<true, true><<<g, 256, 0, st>>>(A, g_batch.stride, g_bank); else k_rot_many<true, false><<<g, 256, 0, st>>>(A, g_batch.stride, g_bank); }
+    else if (g_inline) k_rot_many<false, true><<<g, 256, 0, st>>>(A, g_batch.stride, g_bank);
+    else k_rot_many<false, false><<<g, 256, 0, st>>>(A, g_batch.stride, g_bank);
     CUDA_OK(cudaGetLastError());
     return 0;
+  }
+  template <int NOUT> void wsum_ip(dim3 g, const WsumIpArgs &A, bool bank) {
+    if (bank) { if (g_inline) k_rot_wsum_ip<NOUT, true, true><<<g, 128, 0, st>>>(A, g_batch.stride, g_bank); else k_rot_wsum_ip<NOUT, true, false><<<g, 128, 0, st>>>(A, g_batch.stride, g_bank); }
+    else if (g_inline) k_rot_wsum_ip<NOUT, false, true><<<g, 128, 0, st>>>(A, g_batch.stride, g_bank);
+    else k_rot_wsum_ip<NOUT, false, false><<<g, 128, 0, st>>>(A, g_batch.stride, g_bank);
   }
   int rot_wsum_ip(const WsumIpArgs &A) {
     count();
     const dim3 g(A.N / 2 / 128, A.ell + 1, g_batch.batch);   // N >= 1024
     const bool bank = g_bank.tenant != nullptr;
-    switch (A.nout * 2 + bank) {
-      case 2: k_rot_wsum_ip<1, false><<<g, 128, 0, st>>>(A, g_batch.stride, g_bank); break;
-      case 3: k_rot_wsum_ip<1, true><<<g, 128, 0, st>>>(A, g_batch.stride, g_bank); break;
-      case 4: k_rot_wsum_ip<2, false><<<g, 128, 0, st>>>(A, g_batch.stride, g_bank); break;
-      case 5: k_rot_wsum_ip<2, true><<<g, 128, 0, st>>>(A, g_batch.stride, g_bank); break;
-      case 6: k_rot_wsum_ip<3, false><<<g, 128, 0, st>>>(A, g_batch.stride, g_bank); break;
-      case 7: k_rot_wsum_ip<3, true><<<g, 128, 0, st>>>(A, g_batch.stride, g_bank); break;
-      case 8: k_rot_wsum_ip<4, false><<<g, 128, 0, st>>>(A, g_batch.stride, g_bank); break;
-      case 9: k_rot_wsum_ip<4, true><<<g, 128, 0, st>>>(A, g_batch.stride, g_bank); break;
+    switch (A.nout) {
+      case 1: wsum_ip<1>(g, A, bank); break;
+      case 2: wsum_ip<2>(g, A, bank); break;
+      case 3: wsum_ip<3>(g, A, bank); break;
+      case 4: wsum_ip<4>(g, A, bank); break;
       default: return fail("rotate_wsum: 1..4 output sums");
     }
     CUDA_OK(cudaGetLastError());
@@ -894,6 +909,17 @@ extern "C" int evab_rotate_hoist_const(evab_ctx *c, int ell, uint64_t elt, const
   u32 *perm = nullptr, *ctab = nullptr;
   if (galois_tables(c, elt, &perm, &ctab, "evab_rotate_hoist_const")) return 1;
   BE_BEGIN return hoist_const_impl(be, c->v, ell, ctab, key, out, tmp);
+}
+extern "C" size_t evab_hoist_indicators_bytes(const evab_ctx *c, int n) { return hoist_indicators_elems(c->v, n) * sizeof(u64); }
+extern "C" int evab_hoist_indicators(evab_ctx *c, int n, const uint64_t *elts, uint64_t *out, void *stream) {
+  if (n < 1) return fail("evab_hoist_indicators: n must be >= 1");
+  std::vector<const u32 *> ctabs(n);
+  for (int g = 0; g < n; g++) {
+    u32 *perm = nullptr, *ctab = nullptr;
+    if (galois_tables(c, elts[g], &perm, &ctab, "evab_hoist_indicators")) return 1;
+    ctabs[g] = ctab;
+  }
+  BE_BEGIN return hoist_indicators_impl(be, c->v, n, ctabs.data(), out);
 }
 extern "C" size_t evab_hoist_const_levels_bytes(const evab_ctx *c) { return hoist_levels_words(c->v.k, c->v.N) * sizeof(u64); }
 extern "C" size_t evab_rotate_hoist_const_levels_work_bytes(const evab_ctx *c, int n) { return hoist_const_levels_work_elems(c->v, n) * sizeof(u64); }

@@ -492,9 +492,14 @@ private:
 class B200Server {
 public:
   // maxTenants < 0 or == capacity: tenant id = bank region, filled when the keys are added.  maxTenants > capacity: paging (KeyPager)
-  // rotationKeys: the bank's Galois keys (rotationKeySteps); rotations without a key of their own are composed
-  B200Server(const CKKSParameters &params, int capacity, int device, int maxTenants = -1, const std::string &rotationKeys = "program")
-      : rotationKeys_(rotationKeys) {
+  // rotationKeys: the bank's Galois keys (rotationKeySteps); rotations without a key of their own are composed.
+  // hoistConstants: "stored" -- every region holds the hoist constants of its keys; "inline" -- keys only, the constants are formed
+  // inside the key-switch inner products (KeyBank)
+  B200Server(const CKKSParameters &params, int capacity, int device, int maxTenants = -1, const std::string &rotationKeys = "program",
+             const std::string &hoistConstants = "stored")
+      : rotationKeys_(rotationKeys), hoistConstants_(hoistConstants) {
+    if (hoistConstants != "stored" && hoistConstants != "inline")
+      throw std::invalid_argument("hoist_constants must be \"stored\" or \"inline\", not \"" + hoistConstants + "\"");
     if (maxTenants >= 0 && maxTenants < capacity)
       throw std::invalid_argument("max_tenants (" + std::to_string(maxTenants) + ") is below the number of device slots (capacity " + std::to_string(capacity) + ")");
     const std::vector<int> steps = rotationKeySteps(params, rotationKeys);
@@ -508,7 +513,7 @@ public:
       if (!elt) throw std::invalid_argument("step count too large");
       elts.insert(elt);
     }
-    s->bank = std::make_unique<KeyBank>(s->dev, elts, capacity);
+    s->bank = std::make_unique<KeyBank>(s->dev, elts, capacity, hoistConstants == "inline");
     if (maxTenants > capacity) s->pager = std::make_unique<KeyPager>(s->dev, *s->bank, maxTenants);
     pub_ = std::make_unique<B200Public>(s);
   }
@@ -583,6 +588,7 @@ public:
   B200Public &pub() { return *pub_; }
   const KeyBank &bank() const { return *pub_->shared()->bank; }
   const std::string &rotationKeys() const { return rotationKeys_; }
+  const std::string &hoistConstants() const { return hoistConstants_; }
   std::shared_ptr<Shared> shared() const { return pub_->shared(); }
 
 private:
@@ -592,7 +598,7 @@ private:
     shared()->dev->sync(stream);
     ex.setTenants(slots.data(), (int)slots.size());
   }
-  std::string rotationKeys_;
+  std::string rotationKeys_, hoistConstants_;
   std::unique_ptr<B200Public> pub_;
   std::map<const Executor *, std::vector<int>> staged_;   // device-resident hooks: the tenants staged on a plan replica
 };

@@ -29,28 +29,49 @@ struct KeyBankGuard {
   KeyBankGuard(const std::int32_t *d_tenant, std::size_t stride) { check(evab_set_key_bank(d_tenant, stride)); }
   ~KeyBankGuard() { evab_set_key_bank(nullptr, 0); }
 };
+// scoped evab_set_hoist_inline: the hoisted rotations issued by this thread read indicator rows as their constants
+struct HoistInlineGuard {
+  explicit HoistInlineGuard(bool on) { check(evab_set_hoist_inline(on ? 1 : 0)); }
+  ~HoistInlineGuard() { evab_set_hoist_inline(0); }
+};
 
 // Evaluation keys of up to `capacity` tenants (one client's key set each) in one device allocation.  Every tenant's region has
 // the same layout -- the relinearization key, one Galois key per element of the rotation set, then the hoist constants cadd of
 // every (element, ell) with ell = 1 .. k-1 (one evab_rotate_hoist_const_levels call, when the region is filled) -- so region t's
 // copy of any of them is at region 0's pointer + t * stride() words.  Plans take region 0's pointers and select per instance at
 // run time.  Without paging a tenant id is its region; with paging (KeyPager) the regions are slots that tenants are paged into.
+// Inline hoist constants (inlineConstants): a region holds the keys only, and the bank one copy of every element's indicator rows
+// NTT_m(I_g) [k][N], shared by all tenants; the hoisted rotations form each constant from those rows and the keys they load
+// (evab_set_hoist_inline), so fills compute nothing.
 class KeyBank {
 public:
-  KeyBank(std::shared_ptr<Device> dev, const std::set<u64> &elts, int capacity) : dev_(std::move(dev)), elts_(elts.begin(), elts.end()) {
+  KeyBank(std::shared_ptr<Device> dev, const std::set<u64> &elts, int capacity, bool inlineConstants = false)
+      : dev_(std::move(dev)), elts_(elts.begin(), elts.end()), inline_(inlineConstants) {
     if (capacity < 1 || capacity > 65535) throw std::invalid_argument("key bank capacity must be in [1, 65535]");
     const std::size_t N = dev_->N(), k = (std::size_t)dev_->k();
     if (k < 2) throw std::invalid_argument("a key bank needs at least two primes");
     keyWords_ = (k - 1) * 2 * k * N;
-    for (std::size_t ell = 1; ell < k; ell++) constWords_ += 2 * (ell + 1) * N;
+    if (!inline_)
+      for (std::size_t ell = 1; ell < k; ell++) constWords_ += 2 * (ell + 1) * N;
     stride_ = keyWords_ * (1 + elts_.size()) + constWords_ * elts_.size();
     for (u64 e : elts_) check(evab_galois_prepare(dev_->ctx(), e));
     bank_ = DBuf(dev_, stride_ * (std::size_t)capacity);
     seeds_ = DBuf(dev_, 4 * keys() * (std::size_t)capacity);
-    if (!elts_.empty()) tmp_ = DBuf(dev_, evab_rotate_hoist_const_levels_work_bytes(dev_->ctx(), (int)elts_.size()) / 8);
+    if (!elts_.empty() && !inline_) tmp_ = DBuf(dev_, evab_rotate_hoist_const_levels_work_bytes(dev_->ctx(), (int)elts_.size()) / 8);
+    if (!elts_.empty() && inline_) {
+      ind_ = DBuf(dev_, evab_hoist_indicators_bytes(dev_->ctx(), (int)elts_.size()) / 8);
+      check(evab_hoist_indicators(dev_->ctx(), (int)elts_.size(), elts_.data(), ind_.get(), nullptr));
+    }
     used_.assign(capacity, 0);
     dev_->sync();
   }
+  bool inlineConstants() const { return inline_; }
+  // the indicator rows [k][N] of an element (inline constants; one copy for every tenant)
+  const u64 *indicators(u64 elt) const {
+    if (!inline_) throw std::logic_error("indicator rows are kept by banks with inline hoist constants only");
+    return ind_.get() + index(elt) * (std::size_t)dev_->k() * dev_->N();
+  }
+  std::size_t indicatorBytes() const { return inline_ ? elts_.size() * (std::size_t)dev_->k() * dev_->N() * 8 : 0; }
   int capacity() const { return (int)used_.size(); }
   int tenants() const { return (int)std::count_if(used_.begin(), used_.end(), [](char u) { return u != 0; }); }
   int compressedTenants() const { return (int)std::count(used_.begin(), used_.end(), 2); }
@@ -70,13 +91,14 @@ public:
   const u64 *relin(int t = 0) const { return bank_.get() + (std::size_t)t * stride_; }
   const u64 *galois(u64 elt, int t = 0) const { return relin(t) + keyWords_ * (1 + index(elt)); }
   const u64 *hoistConst(u64 elt, int ell, int t = 0) const {
+    if (inline_) throw std::logic_error("a bank with inline hoist constants stores none");
     if (ell < 1 || ell >= dev_->k()) throw std::invalid_argument("hoist constant level out of range");
     std::size_t off = keyWords_ * (1 + elts_.size()) + constWords_ * index(elt);
     for (int l = 1; l < ell; l++) off += 2 * (std::size_t)(l + 1) * dev_->N();
     return relin(t) + off;
   }
   // copies host images [k-1][2][k][N] (shapes checked by the caller) of the relinearization key and of a Galois key for every
-  // element into a free region and computes its hoist constants; returns the tenant id
+  // element into a free region and computes its hoist constants (stored constants only); returns the tenant id
   int add(const u64 *relinKey, const std::map<u64, const u64 *> &galoisKeys) {
     const auto it = std::find(used_.begin(), used_.end(), 0);
     if (it == used_.end()) throw std::runtime_error("the key bank is full (" + std::to_string(capacity()) + " tenants): remove a tenant first");
@@ -128,10 +150,10 @@ public:
     computeConstants(slot, stream);
   }
   // the hoist constants of every (element, ell) of region `slot` from its Galois keys (one evab_rotate_hoist_const_levels call:
-  // the region's Galois keys and constants are each contiguous, in element order)
+  // the region's Galois keys and constants are each contiguous, in element order); inline constants: nothing to compute
   void computeConstants(int slot, void *stream) {
     fills_++;
-    if (elts_.empty()) return;
+    if (elts_.empty() || inline_) return;
     check(evab_rotate_hoist_const_levels(dev_->ctx(), (int)elts_.size(), elts_.data(), galois(elts_[0], slot), const_cast<u64 *>(hoistConst(elts_[0], 1, slot)),
                                          tmp_.get(), stream));
   }
@@ -146,10 +168,12 @@ private:
   u64 *region(int t) const { return bank_.get() + (std::size_t)t * stride_; }
   std::shared_ptr<Device> dev_;
   std::vector<u64> elts_;                 // sorted
+  bool inline_ = false;                   // inline hoist constants: no constants in the regions, ind_ holds the indicator rows
   std::size_t keyWords_ = 0, constWords_ = 0, stride_ = 0;   // one key; the constants of one element; one tenant
   std::vector<char> used_;                // 0: free, 1: keys added in full, 2: added compressed
   std::uint64_t fills_ = 0;               // regions filled (keys uploaded, constants computed)
   DBuf bank_, tmp_, seeds_;               // seeds_: [region][keys()][32 bytes], the seeds of the region's last compressed fill                       // tmp_: the indicators of computeConstants (fills are ordered on one stream at a time)
+  DBuf ind_;                              // inline constants: [element][k][N] NTT_m(I_g)
 };
 
 class Executor {
@@ -238,6 +262,8 @@ private:
     ws.rotateWsum = [c](int ell, int n, int nout) { return evab_rotate_wsum_work_bytes(c, ell, n, nout); };
     ws.lazyRotsum = [c](int ell, int nout) { return evab_lazy_rotsum_work_bytes(c, ell, nout); };
     ws.encode = [c](int count) { return evab_encode_work_bytes(c, count); };
+    if (bank_ && bank_->inlineConstants() && opt.approxHoist)
+      throw std::invalid_argument("approx_hoist needs stored hoist constants: this server was built with hoist_constants=\"inline\"");
     std::size_t limit = opt.arenaLimit;
     if (!limit) { std::size_t freeB = 0, totalB = 0; check(evab_mem_info(dev_->ctx(), &freeB, &totalB)); limit = freeB; }
     std::set<u64> elts;   // rotations by steps without a key of their own are composed (planner.hpp composeRotations)
@@ -283,7 +309,11 @@ private:
   }
   const u64 *relinKey() const { return bank_ ? bank_->relin() : keys_.relin.get(); }
   const u64 *galoisKey(u64 elt) const { return bank_ ? bank_->galois(elt) : keys_.galois.at(elt).get(); }
-  const u64 *hoistConst(u64 elt, int ell) const { return bank_ ? bank_->hoistConst(elt, ell) : hoistConst_.at(std::make_pair(elt, ell)).get(); }
+  // a hoisted rotation's constant operand: cadd_g at level ell, or with inline constants the element's indicator rows
+  const u64 *hoistConst(u64 elt, int ell) const {
+    if (bank_) return bank_->inlineConstants() ? bank_->indicators(elt) : bank_->hoistConst(elt, ell);
+    return hoistConst_.at(std::make_pair(elt, ell)).get();
+  }
   // the element of the rotation a term applies (a hop of a composed rotation: its term's)
   u64 galoisElt(const Term &t) const {
     const u64 elt = evab_galois_elt_from_step(N_, plan_.stepOf(&t));
@@ -498,6 +528,7 @@ private:
     evab_ctx *c = dev_->ctx();
     BatchGuard bg(p.opt.batch, p.stride, p.rawStride);
     KeyBankGuard kg(bank_ ? reinterpret_cast<const std::int32_t *>(tenantDev_.get()) : nullptr, bank_ ? bank_->stride() : 0);
+    HoistInlineGuard hg(bank_ && bank_->inlineConstants());
     void *forkEv = events_[p.numEvents + p.usedStreams];
     for (int b = 0; p.numFlags && b < p.opt.batch; b++)   // zero-coefficient flags of the shared mod-ups
       check(evab_memset_zero(c, arena_.get() + (std::size_t)b * p.stride + p.flagsOff, 8 * p.numFlags * 8, stream));

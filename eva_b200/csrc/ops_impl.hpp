@@ -322,18 +322,24 @@ template <class BE> int hoist_const_impl(BE &be, const CtxView &c, int ell, cons
   H.ind = tmp; H.key = key; H.out = out; H.primes = c.primes; H.ell = ell; H.k = c.k; H.N = (int)c.N;
   return be.hoist_const(H);
 }
-// cadd_g of every level ell = 1 .. k-1 for n Galois keys [n][k-1][2][k][N] (contiguous), into out [n][ell][2][ell+1][N]: the n
-// indicators, ONE forward transform of all n k rows, one element-wise pass (hoist_levels_elem).  `tmp` holds n k N words
-inline size_t hoist_const_levels_work_elems(const CtxView &c, int n) { return (size_t)n * c.k * c.N; }
-template <class BE>
-int hoist_const_levels_impl(BE &be, const CtxView &c, int n, const u32 *const *ctabs, const u64 *keys, u64 *out, u64 *tmp) {
+// NTT_m(I_g) of n Galois elements for every prime m, into out [n][k][N]: the n indicators, ONE forward transform of all n k rows.
+// The key-independent half of the hoist constants: the inline hoist constants (ks_inner_elem, INL) read these rows directly
+inline size_t hoist_indicators_elems(const CtxView &c, int n) { return (size_t)n * c.k * c.N; }
+template <class BE> int hoist_indicators_impl(BE &be, const CtxView &c, int n, const u32 *const *ctabs, u64 *out) {
   if (c.k < 2) return be.error("hoist constants need at least two primes");
   if (n < 1) return be.error("hoist constants: n must be >= 1");
   for (int g = 0; g < n; g++)
-    if (int rc = be.hoist_indicator(tmp + (size_t)g * c.k * c.N, ctabs[g], (int)c.N, c.k)) return rc;
+    if (int rc = be.hoist_indicator(out + (size_t)g * c.k * c.N, ctabs[g], (int)c.N, c.k)) return rc;
   int pidx[32];
   for (int m = 0; m < c.k; m++) pidx[m] = m;
-  if (int rc = ntt_batch_impl(be, c, false, tmp, (size_t)n * c.k, pidx, c.k)) return rc;
+  return ntt_batch_impl(be, c, false, out, (size_t)n * c.k, pidx, c.k);
+}
+// cadd_g of every level ell = 1 .. k-1 for n Galois keys [n][k-1][2][k][N] (contiguous), into out [n][ell][2][ell+1][N]: the
+// indicator rows (hoist_indicators_impl), one element-wise pass (hoist_levels_elem).  `tmp` holds n k N words
+inline size_t hoist_const_levels_work_elems(const CtxView &c, int n) { return hoist_indicators_elems(c, n); }
+template <class BE>
+int hoist_const_levels_impl(BE &be, const CtxView &c, int n, const u32 *const *ctabs, const u64 *keys, u64 *out, u64 *tmp) {
+  if (int rc = hoist_indicators_impl(be, c, n, ctabs, tmp)) return rc;
   HoistLevelsArgs H;
   H.ind = tmp; H.key = keys; H.out = out; H.primes = c.primes; H.k = c.k; H.N = (int)c.N;
   return be.hoist_levels(H, n);
@@ -376,10 +382,21 @@ int rotate_modup_many_impl(BE &be, const CtxView &c, int ell, int n, u64 *out, c
 inline size_t rotate_wsum_work_elems(const CtxView &c, int ell, int n, int nout) {
   return (size_t)2 * n * 2 * c.N + (size_t)2 * nout * 2 * ell * c.N;
 }
+// inline hoist constants (evab_set_hoist_inline): the backend's hoist_inline() where it has one, else off.  While on, the cadd
+// operands of the hoisted rotations are the elements' indicator rows [k][N] (ks_inner_elem, INL)
+template <class BE> auto hoist_inline_of(BE &be, int) -> decltype(be.hoist_inline()) { return be.hoist_inline(); }
+template <class BE> bool hoist_inline_of(BE &, long) { return false; }
 #if !defined(__CUDACC__)
 // key-bank offset of a replayed instance: the replay backend's key_off() where it has one (evab_set_key_bank), else 0
 template <class BE> auto replay_key_off(BE &be, int) -> decltype(be.key_off()) { return be.key_off(); }
 template <class BE> long long replay_key_off(BE &, long) { return 0; }
+template <int NOUT> void rot_wsum_ip_replay(const WsumIpArgs &A, long long koff, bool inl) {
+  for (int mi = 0; mi <= A.ell; mi++)
+    for (int j = 0; j < A.N; j += 2) {
+      if (inl) rot_wsum_ip_elem<NOUT, true>(A, mi, j, 0, koff);
+      else rot_wsum_ip_elem<NOUT>(A, mi, j, 0, koff);
+    }
+}
 #endif
 // the inner products with the weighting: k_rot_wsum_ip in the CUDA build; compiled without CUDA (the CPU emulator of the tests) the
 // same element body replayed serially on the host
@@ -388,14 +405,14 @@ template <class BE> int rot_wsum_ip_step(BE &be, const WsumIpArgs &A) {
   return be.rot_wsum_ip(A);
 #else
   const long long koff = replay_key_off(be, 0);
-  for (int mi = 0; mi <= A.ell; mi++)
-    for (int j = 0; j < A.N; j += 2) switch (A.nout) {
-        case 1: rot_wsum_ip_elem<1>(A, mi, j, 0, koff); break;
-        case 2: rot_wsum_ip_elem<2>(A, mi, j, 0, koff); break;
-        case 3: rot_wsum_ip_elem<3>(A, mi, j, 0, koff); break;
-        case 4: rot_wsum_ip_elem<4>(A, mi, j, 0, koff); break;
-        default: return be.error("rotate_wsum: 1..4 output sums");
-      }
+  const bool inl = hoist_inline_of(be, 0);
+  switch (A.nout) {
+    case 1: rot_wsum_ip_replay<1>(A, koff, inl); break;
+    case 2: rot_wsum_ip_replay<2>(A, koff, inl); break;
+    case 3: rot_wsum_ip_replay<3>(A, koff, inl); break;
+    case 4: rot_wsum_ip_replay<4>(A, koff, inl); break;
+    default: return be.error("rotate_wsum: 1..4 output sums");
+  }
   return 0;
 #endif
 }
@@ -489,6 +506,7 @@ inline size_t lazy_rotsum_work_elems(const CtxView &c, int ell, int nout) { retu
 template <class BE>
 int lazy_rotsum_impl(BE &be, const CtxView &c, int ell, int nout, u64 *out, const u64 *a, const u64 *ext, int n, const u32 *const *perms,
                      const u64 *const *keys, const u64 *const *cadds, const u64 *const *wts, u64 *work) {
+  if (hoist_inline_of(be, 0)) return be.error("lazy_rotsum (approx_hoist) takes stored hoist constants: turn evab_set_hoist_inline off");
   if (ell < 1 || ell > c.k - 1) return be.error("lazy_rotsum needs 1 <= ell <= k-1");
   if (n < 1 || n > LRS_MAX) return be.error("lazy_rotsum: 1..16 rotations");
   if (nout < 1 || nout > LRS_OUT) return be.error("lazy_rotsum: 1..4 output sums");

@@ -169,13 +169,31 @@ struct IpArgs {
   const u64 *cadd;
   int ell, k, N;
 };
+// ---- inline hoist constants (INL = true; evab_set_hoist_inline): the `cadd` operand of a hoisted rotation is read as the element's
+// indicator rows ind [k][N] = NTT_m(I_g) for every prime m (row(m): m for a q row, k - 1 for P) instead of cadd_g, and the constant
+// is formed from the key words the inner product loads anyway:
+//   cadd_g[c][m] = reduce128(S_c) (.) ind[row(m)],   S_c = sum_{J < ell} (q_J mod m) key[J][c][row(m)]     (128 bits)
+// -- hoist_levels_elem's arithmetic (the canonical reduction of the same 128-bit sum, the same mulmod_p), so the same word.  The
+// J = row term is zero (q_m mod q_m) and skipped.  The indicator rows do not depend on the tenant: the key-bank offset is never
+// applied to them.  q_J mod m by Barrett (barrett64 is exact for any 64-bit input); a sum has at most k - 2 <= 22 products below
+// 2^120 (both factors below m < 2^60): below 2^125.
+EVAB_HD u64 q_mod(const PrimeDev *primes, int J, const PrimeDev &P) { return barrett64(primes[J].p, P.p, P.ratio64); }
+// cadd_g[c][m] for both polynomials at coefficients j, j+1 from the sums S_0 = (s0x, s0y), S_1 = (s1x, s1y)
+EVAB_HD void inline_const(const u64 *ind, int row, size_t N, int j, const PrimeDev &P, u64 l0x, u64 h0x, u64 l0y, u64 h0y, u64 l1x, u64 h1x,
+                          u64 l1y, u64 h1y, u64x2 &c0, u64x2 &c1) {
+  const u64x2 ni = ld2(ind + (size_t)row * N + j);
+  c0.x = mulmod_p(reduce128(l0x, h0x, P), ni.x, P); c0.y = mulmod_p(reduce128(l0y, h0y, P), ni.y, P);
+  c1.x = mulmod_p(reduce128(l1x, h1x, P), ni.x, P); c1.y = mulmod_p(reduce128(l1y, h1y, P), ni.y, P);
+}
+
 // off: batch instance offset (words) of t / ext / acc; koff: key offset (words) of the instance's tenant in a key bank
-// (evab_set_key_bank), applied to key and cadd; 0 when all instances share the key
-EVAB_HD void ks_inner_elem(const IpArgs &A, int mi, int j, long long off = 0, long long koff = 0) {
+// (evab_set_key_bank), applied to key and (INL = false) cadd; 0 when all instances share the key
+template <bool INL = false> EVAB_HD void ks_inner_elem(const IpArgs &A, int mi, int j, long long off = 0, long long koff = 0) {
   const int row = (mi == A.ell) ? A.k - 1 : mi;
   const PrimeDev P = A.primes[row];
   const size_t N = A.N;
   u64 l0x = 0, h0x = 0, l0y = 0, h0y = 0, l1x = 0, h1x = 0, l1y = 0, h1y = 0;
+  u64 s0x = 0, t0x = 0, s0y = 0, t0y = 0, s1x = 0, t1x = 0, s1y = 0, t1y = 0;   // INL: S_0, S_1
   for (int J = 0; J < A.ell; J++) {
     u64x2 v;
     if (row == J) {
@@ -191,13 +209,20 @@ EVAB_HD void ks_inner_elem(const IpArgs &A, int mi, int j, long long off = 0, lo
     const u64x2 k1 = ld2(A.key + koff + (((size_t)J * 2 + 1) * A.k + row) * N + j);
     mac128(l0x, h0x, v.x, k0.x); mac128(l0y, h0y, v.y, k0.y);
     mac128(l1x, h1x, v.x, k1.x); mac128(l1y, h1y, v.y, k1.y);
+    if (INL && J != row) {
+      const u64 qj = q_mod(A.primes, J, P);
+      mac128(s0x, t0x, qj, k0.x); mac128(s0y, t0y, qj, k0.y);
+      mac128(s1x, t1x, qj, k1.x); mac128(s1y, t1y, qj, k1.y);
+    }
   }
   u64x2 r0, r1;
   // ext operands may be lazily reduced (< 16p, see EPI_STORE_LAZY): wide reduction
   r0.x = reduce128(l0x, h0x, P); r0.y = reduce128(l0y, h0y, P);
   r1.x = reduce128(l1x, h1x, P); r1.y = reduce128(l1y, h1y, P);
   if (A.cadd) {
-    const u64x2 c0 = ld2(A.cadd + koff + ((size_t)0 * (A.ell + 1) + mi) * N + j), c1 = ld2(A.cadd + koff + ((size_t)1 * (A.ell + 1) + mi) * N + j);
+    u64x2 c0, c1;
+    if (INL) inline_const(A.cadd, row, N, j, P, s0x, t0x, s0y, t0y, s1x, t1x, s1y, t1y, c0, c1);
+    else { c0 = ld2(A.cadd + koff + ((size_t)0 * (A.ell + 1) + mi) * N + j); c1 = ld2(A.cadd + koff + ((size_t)1 * (A.ell + 1) + mi) * N + j); }
     r0.x = addmod(r0.x, c0.x, P.p); r0.y = addmod(r0.y, c0.y, P.p);
     r1.x = addmod(r1.x, c1.x, P.p); r1.y = addmod(r1.y, c1.y, P.p);
   }
@@ -224,13 +249,15 @@ struct RotManyArgs {
   const PrimeDev *primes;
   int n, ell, k, N;
 };
-// koff: key offset of the instance's tenant (ks_inner_elem), applied to key[i] and cadd[i]
-EVAB_HD void rot_many_elem(const RotManyArgs &A, int i, int mi, int j, long long off = 0, long long koff = 0) {
+// koff: key offset of the instance's tenant (ks_inner_elem), applied to key[i] and (INL = false) cadd[i]; INL: cadd[i] is the
+// element's indicator rows (ks_inner_elem)
+template <bool INL = false> EVAB_HD void rot_many_elem(const RotManyArgs &A, int i, int mi, int j, long long off = 0, long long koff = 0) {
   const int row = (mi == A.ell) ? A.k - 1 : mi;
   const PrimeDev P = A.primes[row];
   const size_t N = A.N;
   const u32 pj0 = EVAB_LDG(A.perm[i] + j), pj1 = EVAB_LDG(A.perm[i] + j + 1);
   u64 l0x = 0, h0x = 0, l0y = 0, h0y = 0, l1x = 0, h1x = 0, l1y = 0, h1y = 0;
+  u64 s0x = 0, t0x = 0, s0y = 0, t0y = 0, s1x = 0, t1x = 0, s1y = 0, t1y = 0;   // INL: S_0, S_1
   for (int J = 0; J < A.ell; J++) {
     const u64 *src = (row == J) ? A.t + off + (size_t)J * N : A.ext + off + ((size_t)mi * A.ell + J) * N;
     const u64 vx = EVAB_LDG(src + pj0), vy = EVAB_LDG(src + pj1);
@@ -238,8 +265,15 @@ EVAB_HD void rot_many_elem(const RotManyArgs &A, int i, int mi, int j, long long
     const u64x2 k1 = ld2(A.key[i] + koff + (((size_t)J * 2 + 1) * A.k + row) * N + j);
     mac128(l0x, h0x, vx, k0.x); mac128(l0y, h0y, vy, k0.y);
     mac128(l1x, h1x, vx, k1.x); mac128(l1y, h1y, vy, k1.y);
+    if (INL && J != row) {
+      const u64 qj = q_mod(A.primes, J, P);
+      mac128(s0x, t0x, qj, k0.x); mac128(s0y, t0y, qj, k0.y);
+      mac128(s1x, t1x, qj, k1.x); mac128(s1y, t1y, qj, k1.y);
+    }
   }
-  const u64x2 c0 = ld2(A.cadd[i] + koff + ((size_t)0 * (A.ell + 1) + mi) * N + j), c1 = ld2(A.cadd[i] + koff + ((size_t)1 * (A.ell + 1) + mi) * N + j);
+  u64x2 c0, c1;
+  if (INL) inline_const(A.cadd[i], row, N, j, P, s0x, t0x, s0y, t0y, s1x, t1x, s1y, t1y, c0, c1);
+  else { c0 = ld2(A.cadd[i] + koff + ((size_t)0 * (A.ell + 1) + mi) * N + j); c1 = ld2(A.cadd[i] + koff + ((size_t)1 * (A.ell + 1) + mi) * N + j); }
   u64x2 r0, r1;
   r0.x = addmod(reduce128(l0x, h0x, P), c0.x, P.p); r0.y = addmod(reduce128(l0y, h0y, P), c0.y, P.p);
   r1.x = addmod(reduce128(l1x, h1x, P), c1.x, P.p); r1.y = addmod(reduce128(l1y, h1y, P), c1.y, P.p);
@@ -352,8 +386,9 @@ struct WsumIpArgs {
 // coefficients j, j+1 of row mi (q_0 .. q_{ell-1}, P) of both polynomials, every rotation and every output (nout == NOUT).  acc_i is
 // rot_many_elem's canonical value: the inner product through perm_i + cadd_i, and on a q row + perm_i(P c0) = (P mod q_m) c0[perm_i(j)],
 // read from c0 directly.  A P row is stored; a q row is weighted into A, which then takes the taps.
-// koff: key offset of the instance's tenant (ks_inner_elem), applied to key[i] and cadd[i]
-template <int NOUT> EVAB_HD void rot_wsum_ip_elem(const WsumIpArgs &A, int mi, int j, long long off = 0, long long koff = 0) {
+// koff: key offset of the instance's tenant (ks_inner_elem), applied to key[i] and (INL = false) cadd[i]; INL: cadd[i] is the
+// element's indicator rows (ks_inner_elem)
+template <int NOUT, bool INL = false> EVAB_HD void rot_wsum_ip_elem(const WsumIpArgs &A, int mi, int j, long long off = 0, long long koff = 0) {
   const bool qrow = mi < A.ell;
   const int row = qrow ? mi : A.k - 1;
   const PrimeDev P = A.primes[row];
@@ -370,6 +405,7 @@ template <int NOUT> EVAB_HD void rot_wsum_ip_elem(const WsumIpArgs &A, int mi, i
     const u32 p0 = pj0, p1 = pj1;
     if (i + 1 < A.n) { pj0 = EVAB_LDG(A.perm[i + 1] + j); pj1 = EVAB_LDG(A.perm[i + 1] + j + 1); }   // the next gather's addresses
     u64 l0x = 0, h0x = 0, l0y = 0, h0y = 0, l1x = 0, h1x = 0, l1y = 0, h1y = 0;
+    u64 s0x = 0, t0x = 0, s0y = 0, t0y = 0, s1x = 0, t1x = 0, s1y = 0, t1y = 0;   // INL: S_0, S_1
     for (int J = 0; J < A.ell; J++) {
       const u64 *src = (row == J) ? A.t + off + (size_t)J * N : A.ext + off + ((size_t)mi * A.ell + J) * N;
       const u64 vx = EVAB_LDG(src + p0), vy = EVAB_LDG(src + p1);
@@ -377,8 +413,15 @@ template <int NOUT> EVAB_HD void rot_wsum_ip_elem(const WsumIpArgs &A, int mi, i
       const u64x2 k1 = ld2(A.key[i] + koff + (((size_t)J * 2 + 1) * A.k + row) * N + j);
       mac128(l0x, h0x, vx, k0.x); mac128(l0y, h0y, vy, k0.y);
       mac128(l1x, h1x, vx, k1.x); mac128(l1y, h1y, vy, k1.y);
+      if (INL && J != row) {
+        const u64 qj = q_mod(A.primes, J, P);
+        mac128(s0x, t0x, qj, k0.x); mac128(s0y, t0y, qj, k0.y);
+        mac128(s1x, t1x, qj, k1.x); mac128(s1y, t1y, qj, k1.y);
+      }
     }
-    const u64x2 c0 = ld2(A.cadd[i] + koff + ((size_t)0 * (A.ell + 1) + mi) * N + j), c1 = ld2(A.cadd[i] + koff + ((size_t)1 * (A.ell + 1) + mi) * N + j);
+    u64x2 c0, c1;
+    if (INL) inline_const(A.cadd[i], row, N, j, P, s0x, t0x, s0y, t0y, s1x, t1x, s1y, t1y, c0, c1);
+    else { c0 = ld2(A.cadd[i] + koff + ((size_t)0 * (A.ell + 1) + mi) * N + j); c1 = ld2(A.cadd[i] + koff + ((size_t)1 * (A.ell + 1) + mi) * N + j); }
     u64x2 r0, r1;
     r0.x = addmod(reduce128(l0x, h0x, P), c0.x, P.p); r0.y = addmod(reduce128(l0y, h0y, P), c0.y, P.p);
     r1.x = addmod(reduce128(l1x, h1x, P), c1.x, P.p); r1.y = addmod(reduce128(l1y, h1y, P), c1.y, P.p);

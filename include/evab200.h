@@ -94,6 +94,12 @@ int evab_set_batch(int batch, size_t stride_words, size_t value_stride);
  * layout.  The table is device memory read when the kernels run, so a captured graph
  * follows a table rewritten (stream-ordered) before its launch. */
 int evab_set_key_bank(const int32_t *d_tenant_of_instance, size_t tenant_stride_words);
+/* Inline hoist constants, thread-local like evab_set_key_bank (on != 0: on).  While on, the d_cadd / d_cadds[i] arguments of
+ * evab_rotate_modup_prepared, evab_rotate_modup_many and evab_rotate_wsum are read as the Galois element's indicator rows
+ * [k][N] (evab_hoist_indicators) instead of its hoist constant, the constant being formed inside the key-switch inner product
+ * from the key rows it loads (same bits); those rows are shared by all tenants of a key bank and are NOT shifted by the
+ * key-bank offset.  evab_lazy_rotsum fails while it is on. */
+int evab_set_hoist_inline(int on);
 /* number of kernel launches issued through this context so far */
 uint64_t evab_launch_count(const evab_ctx *ctx);
 
@@ -216,6 +222,11 @@ size_t evab_hoist_const_levels_bytes(const evab_ctx *ctx);
 size_t evab_rotate_hoist_const_levels_work_bytes(const evab_ctx *ctx, int n);
 int evab_rotate_hoist_const_levels(evab_ctx *ctx, int n, const uint64_t *galois_elts, const uint64_t *d_keys, uint64_t *d_out, uint64_t *d_tmp,
                                    void *stream);
+/* The key-independent half of the hoist constants: d_out [n][k][N] receives NTT_m(I_g) for every prime m of the n Galois elements
+ * (each prepared with evab_galois_prepare), I_g the indicator of the coefficients the automorphism negates -- the rows that
+ * evab_rotate_hoist_const_levels multiplies by the key sums, and that evab_set_hoist_inline reads.  Stream-ordered. */
+size_t evab_hoist_indicators_bytes(const evab_ctx *ctx, int n);
+int evab_hoist_indicators(evab_ctx *ctx, int n, const uint64_t *galois_elts, uint64_t *d_out, void *stream);
 /* Seed-compressed key-switch keys: a key whose c1 rows (the uniform halves) are not stored but expanded from a 32-byte seed by
  * the rule of eva_b200/csrc/key_expand.cuh (ChaCha20 blocks keyed by the seed, rejection sampling mod q; DESIGN §2).  Writes the
  * c1 rows of n keys d_keys [n][k-1][2][k][N]: row (J, m) of key g from the seed d_seeds[g] (device, [n][32] bytes) modulo
