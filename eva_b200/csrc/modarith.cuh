@@ -142,11 +142,25 @@ EVAB_HD u64 madw32(u32 a, u32 b, u64 c) {
   return (u64)a * b + c;
 #endif
 }
+// a * b + (ch:cl), the addend given as its two 32-bit halves, as a carry-chained mad.lo.cc / madc.hi pair.  Written as
+// mad.wide.u32 with an addend that is not itself a wide product, ptxas emits IMAD.WIDE + IADD3 + IMAD.X; from this form it
+// emits one IMAD.WIDE with the halves as a register-pair addend (fold_mul, fold61, fold_canon: 8-11 % fewer instructions
+// in the N = 16384 transforms, tools/ntt_sass_report.py).
+EVAB_HD u64 madc32(u32 a, u32 b, u32 cl, u32 ch) {
+#if defined(__CUDA_ARCH__)
+  u32 rl, rh; u64 r;
+  asm("mad.lo.cc.u32 %0, %2, %3, %4;\n\tmadc.hi.u32 %1, %2, %3, %5;" : "=r"(rl), "=r"(rh) : "r"(a), "r"(b), "r"(cl), "r"(ch));
+  asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "r"(rl), "r"(rh));
+  return r;
+#else
+  return (u64)a * b + (((u64)ch << 32) | cl);
+#endif
+}
 // any u64 -> congruent value < 2^61 + 7*eps
-EVAB_HD u64 fold61(u64 x, u32 eps) { return madw32((u32)(x >> 61), eps, x & ((1ull << 61) - 1)); }
+EVAB_HD u64 fold61(u64 x, u32 eps) { return madc32((u32)(x >> 61), eps, (u32)x, (u32)(x >> 32) & 0x1fffffffu); }
 // x < 16p -> canonical [0,p): x = h*2^60 + l == l + h*delta, which is < p + 2^29; one conditional subtraction
 EVAB_HD u64 fold_canon(u64 x, u32 eps, u64 p) {
-  return csub(madw32((u32)(x >> 60), eps >> 1, x & ((1ull << 60) - 1)), p);
+  return csub(madc32((u32)(x >> 60), eps >> 1, (u32)x, (u32)(x >> 32) & 0x0fffffffu), p);
 }
 EVAB_HD u64 fold_mul(u64 y, u64 w, u64 v, u32 eps) {
   const u32 y0 = (u32)y, y1 = (u32)(y >> 32);
@@ -165,8 +179,7 @@ EVAB_HD u64 fold_mul(u64 y, u64 w, u64 v, u32 eps) {
       : "=r"(s0), "=r"(s1), "=r"(s2)
       : "r"((u32)A), "r"((u32)(A >> 32)), "r"((u32)A2), "r"((u32)(A2 >> 32)), "r"((u32)B), "r"((u32)(B >> 32)));
   asm("shf.l.wrap.b32 %0, %1, %2, 3;" : "=r"(H) : "r"(s1), "r"(s2));
-  u64 L; asm("mov.b64 %0, {%1, %2};" : "=l"(L) : "r"(s0), "r"(s1 & 0x1fffffffu));
-  return madw32(H, eps, 0) + L;
+  return madc32(H, eps, s0, s1 & 0x1fffffffu);   // (S mod 2^61) + (S >> 61) * eps
 #else
   const unsigned __int128 S = (unsigned __int128)y0 * w + (unsigned __int128)y1 * v;
   return (u64)(S & ((1ull << 61) - 1)) + (u64)(S >> 61) * eps;

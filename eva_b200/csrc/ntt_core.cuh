@@ -369,9 +369,10 @@ struct FoldP { u64 p, p3, p8; u32 eps; };
 template <class FPr> EVAB_HD FoldP fold_params(const FPr &P) { FoldP F; F.p = P.p; F.p3 = P.p3; F.p8 = P.p8; F.eps = P.eps; return F; }
 
 template <int D> EVAB_HD void ffwd_stage(u64 (&x)[NTT_E], int (&bb)[NTT_E], const u64x2 *tw, u32 tw0, const FoldP &F) {
+  const u64x2 *twg = tw + (size_t)tw0;   // the stage's first group, addressed once; the groups are immediate offsets from it
 #pragma unroll
   for (int g = 0; g < NTT_E / 2 / D; g++) {
-    const u64x2 w = ldg_tw(tw + tw0 + g);
+    const u64x2 w = ldg_tw(twg + g);
 #pragma unroll
     for (int j = 0; j < D; j++) {
       const int k = g * 2 * D + j;
@@ -432,9 +433,10 @@ EVAB_HD void finv_bfly(u64 &xa, u64 &xb, int &ba, int &bby, const u64x2 &w, cons
   EVAB_CHECK_BOUND(X, bx, F); EVAB_CHECK_BOUND(Y, by, F); EVAB_CHECK_BOUND(xa, ba, F); EVAB_CHECK_BOUND(xb, bby, F);
 }
 template <int D> EVAB_HD void finv_stage(u64 (&x)[NTT_E], int (&bb)[NTT_E], const u64x2 *tw, u32 tw0, const FoldP &F) {
+  const u64x2 *twg = tw + (size_t)tw0;   // as in ffwd_stage
 #pragma unroll
   for (int g = 0; g < NTT_E / 2 / D; g++) {
-    const u64x2 w = ldg_tw(tw + tw0 + g);
+    const u64x2 w = ldg_tw(twg + g);
 #pragma unroll
     for (int j = 0; j < D; j++) {
       const int k = g * 2 * D + j;
