@@ -72,6 +72,12 @@ extern "C" int evab_set_hoist_inline(int on) {
   g_inline = on != 0;
   return 0;
 }
+// thread-local seeded keys (evab_set_key_seeded): the key operands of the key switches are seeded images, c1 drawn in the kernels
+static thread_local bool g_seeded = false;
+extern "C" int evab_set_key_seeded(int on) {
+  g_seeded = on != 0;
+  return 0;
+}
 
 
 // ---------------------------------------------------------------------------
@@ -214,27 +220,38 @@ __global__ void __launch_bounds__(256) k_sum_terms(const SumArgs A, const long l
 }
 // key offset of this block's instance: BANK = false is the shared-key launch (offset 0, the table is not read)
 template <bool BANK> __device__ __forceinline__ long long key_off(const KeyBankSel &K) { return BANK ? (long long)__ldg(K.tenant + blockIdx.z) * K.stride : 0; }
-// INL: inline hoist constants (ks_inner_elem)
-template <bool BANK, bool INL> __global__ void __launch_bounds__(256) k_ks_inner(const IpArgs A, const long long bstride, const KeyBankSel K) {
+// SEED: the c1 tile of a seeded key, [ell][2 blockDim.x] words of dynamic shared memory (seed_tile_bytes; ops_kernels.cuh SeedTileDev)
+__device__ __forceinline__ SeedTileDev seed_tile() {
+  extern __shared__ __align__(16) u64 sm[];
+  return SeedTileDev{sm};
+}
+// INL: inline hoist constants (ks_inner_elem); SEED: seeded key images (every launch has N / 512 blocks per row or a multiple of
+// them, so the tile loop is uniform over the block)
+template <bool BANK, bool INL, bool SEED> __global__ void __launch_bounds__(256) k_ks_inner(const IpArgs A, const long long bstride, const KeyBankSel K) {
   const long long off = (long long)blockIdx.z * bstride;   // parameters stay in constant memory: no local copy
   const long long koff = key_off<BANK>(K);
+  SeedTileDev tile = seed_tile();
   for (int j = (blockIdx.x * blockDim.x + threadIdx.x) * 2; j < A.N; j += gridDim.x * blockDim.x * 2)
-    ks_inner_elem<INL>(A, blockIdx.y, j, off, koff);
+    ks_inner_elem<INL, SEED>(A, blockIdx.y, j, off, koff, SEED ? &tile : nullptr);
 }
 __global__ void __launch_bounds__(256) k_scale_c0(const u64 *c0, u64 *ext, const PrimeDev *primes, int ell, int k, int N, const long long bstride) {
   const long long off = (long long)blockIdx.z * bstride;
   for (int j = blockIdx.x * blockDim.x + threadIdx.x; j < N; j += gridDim.x * blockDim.x) scale_c0_elem(c0, ext, primes, ell, k, N, blockIdx.y, j, off);
 }
 // INL: 3 blocks per SM (80 registers) -- at 4 the inline instance spills about 100 bytes
-template <bool BANK, bool INL> __global__ void __launch_bounds__(256, INL ? 3 : 4) k_rot_many(const RotManyArgs A, const long long bstride, const KeyBankSel K) {
+template <bool BANK, bool INL, bool SEED> __global__ void __launch_bounds__(256, INL ? 3 : 4) k_rot_many(const RotManyArgs A, const long long bstride, const KeyBankSel K) {
   const long long off = (long long)blockIdx.z * bstride, koff = key_off<BANK>(K);
   const int i = blockIdx.y / (A.ell + 1), mi = blockIdx.y % (A.ell + 1);
-  for (int j = (blockIdx.x * blockDim.x + threadIdx.x) * 2; j < A.N; j += gridDim.x * blockDim.x * 2) rot_many_elem<INL>(A, i, mi, j, off, koff);
+  SeedTileDev tile = seed_tile();
+  for (int j = (blockIdx.x * blockDim.x + threadIdx.x) * 2; j < A.N; j += gridDim.x * blockDim.x * 2)
+    rot_many_elem<INL, SEED>(A, i, mi, j, off, koff, SEED ? &tile : nullptr);
 }
 // grid.y = row of the extended basis; every thread loops over the rotations, so blocks are kept small for more of them
-template <int NOUT, bool BANK, bool INL> __global__ void __launch_bounds__(128) k_rot_wsum_ip(const WsumIpArgs A, const long long bstride, const KeyBankSel K) {
+template <int NOUT, bool BANK, bool INL, bool SEED> __global__ void __launch_bounds__(128) k_rot_wsum_ip(const WsumIpArgs A, const long long bstride, const KeyBankSel K) {
   const long long off = (long long)blockIdx.z * bstride, koff = key_off<BANK>(K);
-  for (int j = (blockIdx.x * blockDim.x + threadIdx.x) * 2; j < A.N; j += gridDim.x * blockDim.x * 2) rot_wsum_ip_elem<NOUT, INL>(A, blockIdx.y, j, off, koff);
+  SeedTileDev tile = seed_tile();
+  for (int j = (blockIdx.x * blockDim.x + threadIdx.x) * 2; j < A.N; j += gridDim.x * blockDim.x * 2)
+    rot_wsum_ip_elem<NOUT, INL, SEED>(A, blockIdx.y, j, off, koff, SEED ? &tile : nullptr);
 }
 // grid.y = (polynomial, residue) of the outputs
 __global__ void __launch_bounds__(256) k_rot_wsum(const WsumArgs A, const long long bstride) {
@@ -415,11 +432,39 @@ template <int LOGN> static int launch_inv_t(const NttLaunch &L, size_t jobs, cud
   return fold ? launch_inv_a<LOGN, 1>(L, jobs, st, cluster) : launch_inv_a<LOGN, 0>(L, jobs, st, cluster);
 }
 
+// bytes of a seeded launch's c1 tile: [ell][2 threads] words
+static size_t seed_tile_bytes(int ell, int threads) { return (size_t)ell * 2 * threads * sizeof(u64); }
+// the largest dynamic shared memory a seeded instance needs on a context of k primes (ell = k - 1), allowed once per device and
+// never lowered (contexts of different k share the device).  The 128-thread k_rot_wsum_ip tile stays under the 48 KB default for
+// every k <= 24 (47 104 bytes at ell = 23); the 256-thread k_ks_inner and k_rot_many tiles pass it from ell = 13
+template <class Kern> static int seed_smem_allow(Kern kern, size_t bytes) {
+  if (bytes <= 48 * 1024) return 0;
+  cudaFuncAttributes fa;
+  CUDA_OK(cudaFuncGetAttributes(&fa, kern));
+  if ((size_t)fa.maxDynamicSharedSizeBytes < bytes) CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
+  return 0;
+}
+static int seeded_smem_opt_in(int k) {
+  static std::mutex mu;
+  std::lock_guard<std::mutex> lock(mu);
+  const size_t b = seed_tile_bytes(k - 1, 256);
+  if (seed_smem_allow(k_ks_inner<false, false, true>, b) || seed_smem_allow(k_ks_inner<false, true, true>, b) ||
+      seed_smem_allow(k_ks_inner<true, false, true>, b) || seed_smem_allow(k_ks_inner<true, true, true>, b) ||
+      seed_smem_allow(k_rot_many<false, true, true>, b) || seed_smem_allow(k_rot_many<true, true, true>, b))
+    return 1;
+  static_assert(24 * 2 * 128 * sizeof(u64) <= 48 * 1024, "the k_rot_wsum_ip seeded tile fits the default shared memory");
+  return 0;
+}
+
 struct CudaBE {
   const evab_ctx *c;
   cudaStream_t st;
   int error(const char *m) { return fail(m); }
   bool hoist_inline() const { return g_inline; }
+  bool key_seeded() const { return g_seeded; }
+  // dynamic shared memory of a seeded launch (the c1 tile, SeedTileDev); the instances whose tile can pass the 48 KB default were
+  // allowed their largest one when the context was created (seeded_smem_opt_in), so a launch -- or a graph capture -- sets nothing
+  static size_t seed_smem(int ell, int threads) { return seed_tile_bytes(ell, threads); }
   void count(unsigned n = 1) const { c->launches.fetch_add(n, std::memory_order_relaxed); }
   dim3 grid(int rows, int per_thread = 2) const {
     int per_row = (int)(c->v.N / per_thread / 256);
@@ -478,13 +523,21 @@ struct CudaBE {
     CUDA_OK(cudaGetLastError());
     return 0;
   }
+  template <bool BANK> void inner_seeded(dim3 g, const IpArgs &A, bool inl) {
+    if (inl) k_ks_inner<BANK, true, true><<<g, 256, seed_smem(A.ell, 256), st>>>(A, g_batch.stride, g_bank);
+    else k_ks_inner<BANK, false, true><<<g, 256, seed_smem(A.ell, 256), st>>>(A, g_batch.stride, g_bank);
+  }
   int inner(const IpArgs &A) {
     count();
     const dim3 g = grid(A.ell + 1);
     const bool inl = g_inline && A.cadd;   // only the hoisted form has a constant to form
-    if (g_bank.tenant) { if (inl) k_ks_inner<true, true><<<g, 256, 0, st>>>(A, g_batch.stride, g_bank); else k_ks_inner<true, false><<<g, 256, 0, st>>>(A, g_batch.stride, g_bank); }
-    else if (inl) k_ks_inner<false, true><<<g, 256, 0, st>>>(A, g_batch.stride, g_bank);
-    else k_ks_inner<false, false><<<g, 256, 0, st>>>(A, g_batch.stride, g_bank);
+    if (g_seeded) {
+      if (g_bank.tenant) inner_seeded<true>(g, A, inl);
+      else inner_seeded<false>(g, A, inl);
+    }
+    else if (g_bank.tenant) { if (inl) k_ks_inner<true, true, false><<<g, 256, 0, st>>>(A, g_batch.stride, g_bank); else k_ks_inner<true, false, false><<<g, 256, 0, st>>>(A, g_batch.stride, g_bank); }
+    else if (inl) k_ks_inner<false, true, false><<<g, 256, 0, st>>>(A, g_batch.stride, g_bank);
+    else k_ks_inner<false, false, false><<<g, 256, 0, st>>>(A, g_batch.stride, g_bank);
     CUDA_OK(cudaGetLastError());
     return 0;
   }
@@ -497,16 +550,24 @@ struct CudaBE {
   int rot_many(const RotManyArgs &A) {
     count();
     const dim3 g = grid(A.n * (A.ell + 1));
-    if (g_bank.tenant) { if (g_inline) k_rot_many<true, true><<<g, 256, 0, st>>>(A, g_batch.stride, g_bank); else k_rot_many<true, false><<<g, 256, 0, st>>>(A, g_batch.stride, g_bank); }
-    else if (g_inline) k_rot_many<false, true><<<g, 256, 0, st>>>(A, g_batch.stride, g_bank);
-    else k_rot_many<false, false><<<g, 256, 0, st>>>(A, g_batch.stride, g_bank);
+    if (g_seeded) {   // inline constants (require_seeded_inline)
+      if (g_bank.tenant) k_rot_many<true, true, true><<<g, 256, seed_smem(A.ell, 256), st>>>(A, g_batch.stride, g_bank);
+      else k_rot_many<false, true, true><<<g, 256, seed_smem(A.ell, 256), st>>>(A, g_batch.stride, g_bank);
+    }
+    else if (g_bank.tenant) { if (g_inline) k_rot_many<true, true, false><<<g, 256, 0, st>>>(A, g_batch.stride, g_bank); else k_rot_many<true, false, false><<<g, 256, 0, st>>>(A, g_batch.stride, g_bank); }
+    else if (g_inline) k_rot_many<false, true, false><<<g, 256, 0, st>>>(A, g_batch.stride, g_bank);
+    else k_rot_many<false, false, false><<<g, 256, 0, st>>>(A, g_batch.stride, g_bank);
     CUDA_OK(cudaGetLastError());
     return 0;
   }
   template <int NOUT> void wsum_ip(dim3 g, const WsumIpArgs &A, bool bank) {
-    if (bank) { if (g_inline) k_rot_wsum_ip<NOUT, true, true><<<g, 128, 0, st>>>(A, g_batch.stride, g_bank); else k_rot_wsum_ip<NOUT, true, false><<<g, 128, 0, st>>>(A, g_batch.stride, g_bank); }
-    else if (g_inline) k_rot_wsum_ip<NOUT, false, true><<<g, 128, 0, st>>>(A, g_batch.stride, g_bank);
-    else k_rot_wsum_ip<NOUT, false, false><<<g, 128, 0, st>>>(A, g_batch.stride, g_bank);
+    if (g_seeded) {   // inline constants (require_seeded_inline)
+      if (bank) k_rot_wsum_ip<NOUT, true, true, true><<<g, 128, seed_smem(A.ell, 128), st>>>(A, g_batch.stride, g_bank);
+      else k_rot_wsum_ip<NOUT, false, true, true><<<g, 128, seed_smem(A.ell, 128), st>>>(A, g_batch.stride, g_bank);
+    }
+    else if (bank) { if (g_inline) k_rot_wsum_ip<NOUT, true, true, false><<<g, 128, 0, st>>>(A, g_batch.stride, g_bank); else k_rot_wsum_ip<NOUT, true, false, false><<<g, 128, 0, st>>>(A, g_batch.stride, g_bank); }
+    else if (g_inline) k_rot_wsum_ip<NOUT, false, true, false><<<g, 128, 0, st>>>(A, g_batch.stride, g_bank);
+    else k_rot_wsum_ip<NOUT, false, false, false><<<g, 128, 0, st>>>(A, g_batch.stride, g_bank);
   }
   int rot_wsum_ip(const WsumIpArgs &A) {
     count();
@@ -648,6 +709,7 @@ extern "C" int evab_ctx_create(uint64_t N, const uint64_t *primes, int k, int de
   c->ntt_cluster = g_ntt_cluster.load();
   c->primes.assign(primes, primes + k);
   if (ctx_build(c, N, logN, primes, k)) { ctx_free(c); return 1; }   // g_err is set; every partial allocation is released
+  if (k >= 2 && seeded_smem_opt_in(k)) { ctx_free(c); return 1; }
   *out = c;
   return 0;
 }
@@ -910,6 +972,7 @@ extern "C" int evab_rotate_hoist_const(evab_ctx *c, int ell, uint64_t elt, const
   if (galois_tables(c, elt, &perm, &ctab, "evab_rotate_hoist_const")) return 1;
   BE_BEGIN return hoist_const_impl(be, c->v, ell, ctab, key, out, tmp);
 }
+extern "C" size_t evab_seeded_key_bytes(const evab_ctx *c) { return seeded_key_words(c->v.k, c->v.N) * sizeof(u64); }
 extern "C" size_t evab_hoist_indicators_bytes(const evab_ctx *c, int n) { return hoist_indicators_elems(c->v, n) * sizeof(u64); }
 extern "C" int evab_hoist_indicators(evab_ctx *c, int n, const uint64_t *elts, uint64_t *out, void *stream) {
   if (n < 1) return fail("evab_hoist_indicators: n must be >= 1");

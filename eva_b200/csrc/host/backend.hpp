@@ -99,6 +99,7 @@ public:
   // host images [k-1][2][k][N] of the relinearization key and of every element's Galois key (checked by the caller) into a new
   // page-locked block; no device work.  Returns the tenant id
   int add(const u64 *relinKey, const std::map<u64, const u64 *> &galoisKeys) {
+    if (bank_.seededKeys()) throw std::logic_error("a bank of seeded keys takes compressed keys only");
     Block &b = freeBlock(bank_.keyWords(), false);
     const std::size_t kw = bank_.keyWords() / bank_.keys();
     std::memcpy(b.p, relinKey, kw * 8);
@@ -494,12 +495,16 @@ public:
   // maxTenants < 0 or == capacity: tenant id = bank region, filled when the keys are added.  maxTenants > capacity: paging (KeyPager)
   // rotationKeys: the bank's Galois keys (rotationKeySteps); rotations without a key of their own are composed.
   // hoistConstants: "stored" -- every region holds the hoist constants of its keys; "inline" -- keys only, the constants are formed
-  // inside the key-switch inner products (KeyBank)
+  // inside the key-switch inner products (KeyBank).  keyStorage: "expanded" -- every key in full; "seeded" (inline constants only) --
+  // c0 rows and seeds, the key switches draw the c1 rows (KeyBank)
   B200Server(const CKKSParameters &params, int capacity, int device, int maxTenants = -1, const std::string &rotationKeys = "program",
-             const std::string &hoistConstants = "stored")
-      : rotationKeys_(rotationKeys), hoistConstants_(hoistConstants) {
+             const std::string &hoistConstants = "stored", const std::string &keyStorage = "expanded")
+      : rotationKeys_(rotationKeys), hoistConstants_(hoistConstants), keyStorage_(keyStorage) {
     if (hoistConstants != "stored" && hoistConstants != "inline")
       throw std::invalid_argument("hoist_constants must be \"stored\" or \"inline\", not \"" + hoistConstants + "\"");
+    if (keyStorage != "expanded" && !(keyStorage == "seeded" && hoistConstants == "inline"))
+      throw std::invalid_argument("key_storage must be \"expanded\", or \"seeded\" with hoist_constants=\"inline\" (got key_storage=\"" +
+                                  keyStorage + "\", hoist_constants=\"" + hoistConstants + "\")");
     if (maxTenants >= 0 && maxTenants < capacity)
       throw std::invalid_argument("max_tenants (" + std::to_string(maxTenants) + ") is below the number of device slots (capacity " + std::to_string(capacity) + ")");
     const std::vector<int> steps = rotationKeySteps(params, rotationKeys);
@@ -513,12 +518,15 @@ public:
       if (!elt) throw std::invalid_argument("step count too large");
       elts.insert(elt);
     }
-    s->bank = std::make_unique<KeyBank>(s->dev, elts, capacity, hoistConstants == "inline");
+    s->bank = std::make_unique<KeyBank>(s->dev, elts, capacity, hoistConstants == "inline", keyStorage == "seeded");
     if (maxTenants > capacity) s->pager = std::make_unique<KeyPager>(s->dev, *s->bank, maxTenants);
     pub_ = std::make_unique<B200Public>(s);
   }
   // host images [k-1][2][k][N] (shapes checked by the caller); every element of the rotation set must be present
   int addKeys(const u64 *relin, const std::map<u64, const u64 *> &galois) {
+    if (bank().seededKeys())
+      throw std::invalid_argument("this server was built with key_storage=\"seeded\" and takes compressed keys only: add_compressed_keys, or "
+                                  "add_keys of a context whose keys have seeds (generate_keys)");
     for (u64 e : bank().elements())
       if (!galois.count(e)) throw std::invalid_argument("Galois key for element " + std::to_string(e) + " of the server's rotation set is missing");
     std::lock_guard<std::mutex> guard(shared()->execMutex);
@@ -589,6 +597,7 @@ public:
   const KeyBank &bank() const { return *pub_->shared()->bank; }
   const std::string &rotationKeys() const { return rotationKeys_; }
   const std::string &hoistConstants() const { return hoistConstants_; }
+  const std::string &keyStorage() const { return keyStorage_; }
   std::shared_ptr<Shared> shared() const { return pub_->shared(); }
 
 private:
@@ -598,7 +607,7 @@ private:
     shared()->dev->sync(stream);
     ex.setTenants(slots.data(), (int)slots.size());
   }
-  std::string rotationKeys_, hoistConstants_;
+  std::string rotationKeys_, hoistConstants_, keyStorage_;
   std::unique_ptr<B200Public> pub_;
   std::map<const Executor *, std::vector<int>> staged_;   // device-resident hooks: the tenants staged on a plan replica
 };

@@ -34,6 +34,11 @@ struct HoistInlineGuard {
   explicit HoistInlineGuard(bool on) { check(evab_set_hoist_inline(on ? 1 : 0)); }
   ~HoistInlineGuard() { evab_set_hoist_inline(0); }
 };
+// scoped evab_set_key_seeded: the key switches issued by this thread read seeded key images and draw their c1 words
+struct KeySeededGuard {
+  explicit KeySeededGuard(bool on) { check(evab_set_key_seeded(on ? 1 : 0)); }
+  ~KeySeededGuard() { evab_set_key_seeded(0); }
+};
 
 // Evaluation keys of up to `capacity` tenants (one client's key set each) in one device allocation.  Every tenant's region has
 // the same layout -- the relinearization key, one Galois key per element of the rotation set, then the hoist constants cadd of
@@ -43,20 +48,24 @@ struct HoistInlineGuard {
 // Inline hoist constants (inlineConstants): a region holds the keys only, and the bank one copy of every element's indicator rows
 // NTT_m(I_g) [k][N], shared by all tenants; the hoisted rotations form each constant from those rows and the keys they load
 // (evab_set_hoist_inline), so fills compute nothing.
+// Seeded keys (seededKeys, inline constants only): every key of a region is a self-contained seeded image -- its c0 rows [k-1][k][N],
+// then its 32-byte seed padded to 64 bytes (evab_seeded_key_bytes) -- and the key switches draw the c1 rows from the seed
+// (evab_set_key_seeded).  The compressed host image of a tenant is the region's own layout, so a fill is one upload and no launch.
 class KeyBank {
 public:
-  KeyBank(std::shared_ptr<Device> dev, const std::set<u64> &elts, int capacity, bool inlineConstants = false)
-      : dev_(std::move(dev)), elts_(elts.begin(), elts.end()), inline_(inlineConstants) {
+  KeyBank(std::shared_ptr<Device> dev, const std::set<u64> &elts, int capacity, bool inlineConstants = false, bool seededKeys = false)
+      : dev_(std::move(dev)), elts_(elts.begin(), elts.end()), inline_(inlineConstants), seeded_(seededKeys) {
     if (capacity < 1 || capacity > 65535) throw std::invalid_argument("key bank capacity must be in [1, 65535]");
+    if (seeded_ && !inline_) throw std::invalid_argument("a bank of seeded keys forms its hoist constants inline");
     const std::size_t N = dev_->N(), k = (std::size_t)dev_->k();
     if (k < 2) throw std::invalid_argument("a key bank needs at least two primes");
-    keyWords_ = (k - 1) * 2 * k * N;
+    keyWords_ = seeded_ ? evab_seeded_key_bytes(dev_->ctx()) / 8 : (k - 1) * 2 * k * N;
     if (!inline_)
       for (std::size_t ell = 1; ell < k; ell++) constWords_ += 2 * (ell + 1) * N;
     stride_ = keyWords_ * (1 + elts_.size()) + constWords_ * elts_.size();
     for (u64 e : elts_) check(evab_galois_prepare(dev_->ctx(), e));
     bank_ = DBuf(dev_, stride_ * (std::size_t)capacity);
-    seeds_ = DBuf(dev_, 4 * keys() * (std::size_t)capacity);
+    if (!seeded_) seeds_ = DBuf(dev_, 4 * keys() * (std::size_t)capacity);
     if (!elts_.empty() && !inline_) tmp_ = DBuf(dev_, evab_rotate_hoist_const_levels_work_bytes(dev_->ctx(), (int)elts_.size()) / 8);
     if (!elts_.empty() && inline_) {
       ind_ = DBuf(dev_, evab_hoist_indicators_bytes(dev_->ctx(), (int)elts_.size()) / 8);
@@ -66,6 +75,7 @@ public:
     dev_->sync();
   }
   bool inlineConstants() const { return inline_; }
+  bool seededKeys() const { return seeded_; }
   // the indicator rows [k][N] of an element (inline constants; one copy for every tenant)
   const u64 *indicators(u64 elt) const {
     if (!inline_) throw std::logic_error("indicator rows are kept by banks with inline hoist constants only");
@@ -78,8 +88,9 @@ public:
   std::size_t stride() const { return stride_; }                 // words
   std::size_t keys() const { return 1 + elts_.size(); }            // the relinearization key, then a Galois key per element
   std::size_t keyWords() const { return keyWords_ * keys(); }
-  // a compressed tenant's host image: the c0 rows [k-1][k][N] of every key (in region order), then the keys' 32-byte seeds
-  std::size_t compressedWords() const { return keyWords() / 2 + 4 * keys(); }
+  // a compressed tenant's host image: the c0 rows [k-1][k][N] of every key (in region order), then the keys' 32-byte seeds; seeded
+  // keys: the region's keys (seeded images)
+  std::size_t compressedWords() const { return seeded_ ? keyWords() : keyWords() / 2 + 4 * keys(); }
   std::size_t constWords() const { return constWords_ * elts_.size(); }
   const std::vector<u64> &elements() const { return elts_; }
   bool has(u64 elt) const { return std::binary_search(elts_.begin(), elts_.end(), elt); }
@@ -100,6 +111,7 @@ public:
   // copies host images [k-1][2][k][N] (shapes checked by the caller) of the relinearization key and of a Galois key for every
   // element into a free region and computes its hoist constants (stored constants only); returns the tenant id
   int add(const u64 *relinKey, const std::map<u64, const u64 *> &galoisKeys) {
+    if (seeded_) throw std::logic_error("a bank of seeded keys takes compressed keys only");
     const auto it = std::find(used_.begin(), used_.end(), 0);
     if (it == used_.end()) throw std::runtime_error("the key bank is full (" + std::to_string(capacity()) + " tenants): remove a tenant first");
     const int t = (int)(it - used_.begin());
@@ -123,6 +135,17 @@ public:
   }
   // host images [k-1][k][N] of the c0 rows and the seeds of the relinearization key and every element's Galois key -> dst
   void packCompressed(u64 *dst, const u64 *relinC0, const KeySeed &relinSeed, const std::map<u64, std::pair<const u64 *, KeySeed>> &galois) const {
+    if (seeded_) {   // key i: c0 rows then the seed, at i keyWords_
+      const std::size_t w = keyWords_ - 8;
+      auto put = [&](std::size_t i, const u64 *c0, const KeySeed &seed) {
+        std::memcpy(dst + i * keyWords_, c0, w * 8);
+        std::memset(dst + i * keyWords_ + w, 0, 64);
+        std::memcpy(dst + i * keyWords_ + w, seed.data(), 32);
+      };
+      put(0, relinC0, relinSeed);
+      for (std::size_t i = 0; i < elts_.size(); i++) put(1 + i, galois.at(elts_[i]).first, galois.at(elts_[i]).second);
+      return;
+    }
     const std::size_t w = keyWords_ / 2;
     std::memcpy(dst, relinC0, w * 8);
     std::memcpy(dst + keys() * w, relinSeed.data(), 32);
@@ -141,7 +164,13 @@ public:
   }
   // the same from a compressed image: one strided upload puts every c0 row in its place (the digits of all keys are (k-1) keys()
   // rows of k N words, 2 k N words apart in the region), the seeds go to the slot's seed block, one launch expands every c1 row
+  // (seeded keys: the image is the region's keys, one upload)
   void fillCompressed(int slot, const u64 *image, void *stream) {
+    if (seeded_) {
+      dev_->upload(region(slot), image, keyWords() * 8, stream);
+      computeConstants(slot, stream);   // counts the fill; inline constants compute nothing
+      return;
+    }
     const std::size_t kN = (std::size_t)dev_->k() * dev_->N(), rows = keys() * ((std::size_t)dev_->k() - 1);
     check(evab_upload_2d(dev_->ctx(), region(slot), 2 * kN * 8, image, kN * 8, kN * 8, rows, stream));
     u64 *seeds = seeds_.get() + 4 * keys() * (std::size_t)slot;
@@ -169,6 +198,7 @@ private:
   std::shared_ptr<Device> dev_;
   std::vector<u64> elts_;                 // sorted
   bool inline_ = false;                   // inline hoist constants: no constants in the regions, ind_ holds the indicator rows
+  bool seeded_ = false;                   // seeded keys: keyWords_ is one seeded image, no seeds_ (the seeds are in the images)
   std::size_t keyWords_ = 0, constWords_ = 0, stride_ = 0;   // one key; the constants of one element; one tenant
   std::vector<char> used_;                // 0: free, 1: keys added in full, 2: added compressed
   std::uint64_t fills_ = 0;               // regions filled (keys uploaded, constants computed)
@@ -529,6 +559,7 @@ private:
     BatchGuard bg(p.opt.batch, p.stride, p.rawStride);
     KeyBankGuard kg(bank_ ? reinterpret_cast<const std::int32_t *>(tenantDev_.get()) : nullptr, bank_ ? bank_->stride() : 0);
     HoistInlineGuard hg(bank_ && bank_->inlineConstants());
+    KeySeededGuard sg(bank_ && bank_->seededKeys());
     void *forkEv = events_[p.numEvents + p.usedStreams];
     for (int b = 0; p.numFlags && b < p.opt.batch; b++)   // zero-coefficient flags of the shared mod-ups
       check(evab_memset_zero(c, arena_.get() + (std::size_t)b * p.stride + p.flagsOff, 8 * p.numFlags * 8, stream));

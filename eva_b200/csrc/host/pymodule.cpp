@@ -506,17 +506,19 @@ PYBIND11_MODULE(_eva_b200, m) {
                              "Executes compiled programs for many clients: each client's evaluation keys are a tenant of a key bank of fixed "
                              "capacity, the plans are shared by all tenants, and every instance of a batch runs with its own tenant's keys");
   srv.def(py::init([](const CKKSParameters &params, int capacity, int device, std::optional<int> maxTenants, const std::string &rotationKeys,
-                       const std::string &hoistConstants) {
-        return std::make_unique<B200Server>(params, capacity, device, maxTenants ? *maxTenants : -1, rotationKeys, hoistConstants);
+                       const std::string &hoistConstants, const std::string &keyStorage) {
+        return std::make_unique<B200Server>(params, capacity, device, maxTenants ? *maxTenants : -1, rotationKeys, hoistConstants, keyStorage);
       }), py::arg("params"), py::arg("capacity") = 64, py::arg("device") = 0, py::arg("max_tenants") = py::none(), py::arg("rotation_keys") = "program",
-      py::arg("hoist_constants") = "stored",
+      py::arg("hoist_constants") = "stored", py::arg("key_storage") = "expanded",
       "capacity: device slots (key-bank regions).  max_tenants None or == capacity: a tenant id is its slot, filled when its keys are "
       "added.  max_tenants > capacity: up to max_tenants tenants' keys in page-locked host memory, paged into the slots (least "
       "recently used first) as batches need them.  rotation_keys: the Galois keys every tenant supplies -- \"program\", one per "
       "rotation step of the program; \"power_of_two\", one per NAF term of its steps (the other rotations are composed from them, "
       "as SEAL's rotate_vector does).  hoist_constants: \"stored\", every slot also holds the hoist constants of its Galois keys "
       "(computed at every fill); \"inline\", slots hold the keys only and the hoisted rotations form the constants inside the "
-      "key-switch inner product (same outputs, smaller slots; approx_hoist is not available)")
+      "key-switch inner product (same outputs, smaller slots; approx_hoist is not available).  key_storage: \"expanded\", every key in "
+      "full; \"seeded\" (with hoist_constants=\"inline\"), slots hold each key's c0 rows and seed and the key switches draw the uniform "
+      "half from the seed (same outputs, half the slot; compressed keys only)")
       .def("add_raw_keys", [](B200Server &s, const u64arr &relin, const std::map<u64, u64arr> &galois) {
         const std::size_t kk = s.shared()->dev->k(), N = s.shared()->dev->N();
         requireShape(relin, {kk - 1, 2, kk, N}, "relinearization key");
@@ -633,11 +635,12 @@ PYBIND11_MODULE(_eva_b200, m) {
         d["evictions"] = pg ? pg->cache().evictions() : 0;
         d["rotation_keys"] = s.rotationKeys();
         d["hoist_constants"] = s.hoistConstants();
+        d["key_storage"] = s.keyStorage();
         d["indicator_bytes"] = b.indicatorBytes();
         return d;
       }, "capacity / device_slots: key-bank regions; rotation_keys: the key set of galois_elements (\"program\" or \"power_of_two\"); "
          "hoist_constants: \"stored\" or \"inline\" (then hoist_const_bytes_per_tenant is 0 and indicator_bytes the one shared copy of "
-         "the elements' indicator rows); "
+         "the elements' indicator rows); key_storage: \"expanded\" or \"seeded\" (key_bytes_per_tenant then counts c0 rows and seeds); "
          "max_tenants: tenant ids (more than the slots: paging); resident: the tenants "
          "holding a slot; host_key_bytes: page-locked host memory of the paged keys (compressed tenants: c0 rows and seeds); "
          "compressed_tenants: tenants added in compressed form; fills: slots filled (keys uploaded and "

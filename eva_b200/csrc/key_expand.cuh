@@ -66,31 +66,40 @@ struct ExpandArgs {
   uint32_t N, k;
 };
 
+// The reduction of an accepted candidate v < lim is a parameter of the draw: any exact v mod q gives the same value.  KxRem is the
+// rule as written (v % q); the key-switch inner products of seeded keys (ops_kernels.cuh seeded_c1_draw8) pass a Barrett reducer.
+struct KxRem {
+  uint64_t q;
+  EVAB_HD uint64_t operator()(uint64_t v) const { return v % q; }
+};
+
 // coefficient j of row r, rejected in the primary draw: the fallback search
-EVAB_HD uint64_t kx_fallback(const uint32_t *key, uint64_t q, uint64_t lim, uint64_t r, uint32_t j) {
+template <class Red> EVAB_HD uint64_t kx_fallback(const uint32_t *key, const Red &red, uint64_t lim, uint64_t r, uint32_t j) {
   uint32_t w[16];
   uint64_t v = 0;
   for (uint32_t t = 0; t < KX_FALLBACK_BLOCKS; t++) {
     chacha20_block(key, (uint64_t)j * KX_FALLBACK_BLOCKS + t, KX_FALLBACK_NONCE | r, w);
     for (int i = 0; i < 8; i++) {
       v = (uint64_t)w[2 * i] | ((uint64_t)w[2 * i + 1] << 32);
-      if (v < lim) return v % q;
+      if (v < lim) return red(v);
     }
   }
-  return v % q;
+  return red(v);
 }
+EVAB_HD uint64_t kx_fallback(const uint32_t *key, uint64_t q, uint64_t lim, uint64_t r, uint32_t j) { return kx_fallback(key, KxRem{q}, lim, r, j); }
 
-// the rule's draw, shared by key rows and ciphertext rows: coefficients 8 t .. 8 t + 7 of row r (modulus q, lim = kx_limit(q))
+// the rule's draw, shared by key rows and ciphertext rows: coefficients 8 t .. 8 t + 7 of row r (lim = kx_limit(q), red: v mod q)
 // from one primary block, a rejected candidate replaced by its fallback search
-EVAB_HD void kx_draw8(const uint32_t *key, uint64_t r, uint32_t t, uint64_t q, uint64_t lim, uint64_t *v) {
+template <class Red> EVAB_HD void kx_draw8(const uint32_t *key, uint64_t r, uint32_t t, const Red &red, uint64_t lim, uint64_t *v) {
   uint32_t w[16];
   chacha20_block(key, t, r, w);
 #pragma unroll
   for (int i = 0; i < 8; i++) {
     const uint64_t c = (uint64_t)w[2 * i] | ((uint64_t)w[2 * i + 1] << 32);
-    v[i] = c < lim ? c % q : kx_fallback(key, q, lim, r, 8 * t + i);
+    v[i] = c < lim ? red(c) : kx_fallback(key, red, lim, r, 8 * t + i);
   }
 }
+EVAB_HD void kx_draw8(const uint32_t *key, uint64_t r, uint32_t t, uint64_t q, uint64_t lim, uint64_t *v) { kx_draw8(key, r, t, KxRem{q}, lim, v); }
 
 // 8 coefficients to dst (64-byte aligned: N is a multiple of 8 and rows start on 64-byte boundaries): 16-byte stores on the device
 EVAB_HD void kx_store8(uint64_t *dst, const uint64_t *v) {

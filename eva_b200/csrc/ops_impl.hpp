@@ -7,6 +7,9 @@
 #include "ops_kernels.cuh"
 #include "encode_kernels.cuh"
 #include <cstring>
+#if !defined(__CUDACC__)
+#include <vector>
+#endif
 
 struct CtxView {
   u64 N; int logN, k;
@@ -310,9 +313,25 @@ template <class BE> int rotate_modup_scale_c0_impl(BE &be, const CtxView &c, int
   if (ell < 1 || ell > c.k - 1) return be.error("rotate needs 1 <= ell <= k-1");
   return be.scale_c0(a, ext, ell);
 }
+// inline hoist constants (evab_set_hoist_inline): the backend's hoist_inline() where it has one, else off.  While on, the cadd
+// operands of the hoisted rotations are the elements' indicator rows [k][N] (ks_inner_elem, INL)
+template <class BE> auto hoist_inline_of(BE &be, int) -> decltype(be.hoist_inline()) { return be.hoist_inline(); }
+template <class BE> bool hoist_inline_of(BE &, long) { return false; }
+// seeded keys (evab_set_key_seeded): the backend's key_seeded() where it has one, else off.  While on, the key operands of the key
+// switches are seeded images (ops_kernels.cuh seeded_key_words) whose c1 words the inner products draw (SEED); the hoist constants
+// are then formed inline only, and nothing else may read such a key
+template <class BE> auto key_seeded_of(BE &be, int) -> decltype(be.key_seeded()) { return be.key_seeded(); }
+template <class BE> bool key_seeded_of(BE &, long) { return false; }
+// the hoisted rotations take inline hoist constants with seeded keys
+template <class BE> int require_seeded_inline(BE &be) {
+  if (key_seeded_of(be, 0) && !hoist_inline_of(be, 0))
+    return be.error("hoisted rotations with seeded keys (evab_set_key_seeded) need inline hoist constants (evab_set_hoist_inline)");
+  return 0;
+}
 inline size_t hoist_const_elems(const CtxView &c, int ell) { return (size_t)2 * (ell + 1) * c.N; }
 // cadd_g for one Galois key at one level; `tmp` holds (ell + 1) * N words
 template <class BE> int hoist_const_impl(BE &be, const CtxView &c, int ell, const u32 *ctab, const u64 *key, u64 *out, u64 *tmp) {
+  if (key_seeded_of(be, 0)) return be.error("rotate_hoist_const reads expanded keys: turn evab_set_key_seeded off");
   if (ell < 1 || ell > c.k - 1) return be.error("hoisted rotation needs 1 <= ell <= k-1");
   if (int rc = be.hoist_indicator(tmp, ctab, (int)c.N, ell + 1)) return rc;
   int pidx[32];
@@ -339,6 +358,7 @@ template <class BE> int hoist_indicators_impl(BE &be, const CtxView &c, int n, c
 inline size_t hoist_const_levels_work_elems(const CtxView &c, int n) { return hoist_indicators_elems(c, n); }
 template <class BE>
 int hoist_const_levels_impl(BE &be, const CtxView &c, int n, const u32 *const *ctabs, const u64 *keys, u64 *out, u64 *tmp) {
+  if (key_seeded_of(be, 0)) return be.error("rotate_hoist_const_levels reads expanded keys: turn evab_set_key_seeded off");
   if (int rc = hoist_indicators_impl(be, c, n, ctabs, tmp)) return rc;
   HoistLevelsArgs H;
   H.ind = tmp; H.key = keys; H.out = out; H.primes = c.primes; H.k = c.k; H.N = (int)c.N;
@@ -348,6 +368,7 @@ inline size_t rotate_modup_work_elems(const CtxView &c, int ell) { return (size_
 template <class BE>
 int rotate_modup_prepared_impl(BE &be, const CtxView &c, int ell, u64 *out, const u64 *a, const u64 *ext, const u32 *nperm, const u64 *key, const u64 *cadd, u64 *work) {
   if (ell < 1 || ell > c.k - 1) return be.error("rotate needs 1 <= ell <= k-1");
+  if (int rc = require_seeded_inline(be)) return rc;
   u64 *acc = work, *tmp = work + (size_t)2 * (ell + 1) * c.N;
   return ks_finish(be, c, ell, out, a + (size_t)ell * c.N, ext, key, a, 1, acc, tmp, nperm, nperm, cadd);
 }
@@ -360,6 +381,7 @@ int rotate_modup_many_impl(BE &be, const CtxView &c, int ell, int n, u64 *out, c
                            const u64 *const *keys, const u64 *const *cadds, u64 *work) {
   if (ell < 1 || ell > c.k - 1) return be.error("rotate needs 1 <= ell <= k-1");
   if (n < 1 || n > ROTMANY_MAX) return be.error("rotate_modup_many: 1..16 rotations");
+  if (int rc = require_seeded_inline(be)) return rc;
   const long long N = (long long)c.N;
   u64 *acc = work, *tmp = work + (size_t)n * 2 * (ell + 1) * N;
   RotManyArgs A;
@@ -382,20 +404,54 @@ int rotate_modup_many_impl(BE &be, const CtxView &c, int ell, int n, u64 *out, c
 inline size_t rotate_wsum_work_elems(const CtxView &c, int ell, int n, int nout) {
   return (size_t)2 * n * 2 * c.N + (size_t)2 * nout * 2 * ell * c.N;
 }
-// inline hoist constants (evab_set_hoist_inline): the backend's hoist_inline() where it has one, else off.  While on, the cadd
-// operands of the hoisted rotations are the elements' indicator rows [k][N] (ks_inner_elem, INL)
-template <class BE> auto hoist_inline_of(BE &be, int) -> decltype(be.hoist_inline()) { return be.hoist_inline(); }
-template <class BE> bool hoist_inline_of(BE &, long) { return false; }
 #if !defined(__CUDACC__)
 // key-bank offset of a replayed instance: the replay backend's key_off() where it has one (evab_set_key_bank), else 0
 template <class BE> auto replay_key_off(BE &be, int) -> decltype(be.key_off()) { return be.key_off(); }
 template <class BE> long long replay_key_off(BE &, long) { return 0; }
-template <int NOUT> void rot_wsum_ip_replay(const WsumIpArgs &A, long long koff, bool inl) {
-  for (int mi = 0; mi <= A.ell; mi++)
-    for (int j = 0; j < A.N; j += 2) {
+// the CPU replay's seeded-key tiles (SEED; ops_kernels.cuh SeedTileDev on the device): fill() draws, through seeded_c1_draw8, the
+// c1 words of coefficients j0 .. j0 + T - 1 for every J < ell of row `row` of each of the n keys (their images + koff) into
+// [n][ell][T]; the bodies of those coefficients then read them (begin(i, ...) selects key i's tile)
+struct SeedTileHost {
+  static constexpr int T = 256;
+  std::vector<u64> buf;
+  int ell = 0, j0 = 0;
+  const u64 *cur = nullptr;
+  void fill(const u64 *const *keys, int n, long long koff, int ell_, int row, int k, size_t N, const PrimeDev &P, int tile_j0) {
+    ell = ell_; j0 = tile_j0;
+    buf.assign((size_t)n * ell * T, 0);
+    const u64 lim = kx_limit(P.p);
+    for (int i = 0; i < n; i++) {
+      uint32_t seed[8];
+      seeded_seed(keys[i] + koff, k, N, seed);
+      for (int J = 0; J < ell; J++)
+        for (int b = 0; b < T / 8; b++) seeded_c1_draw8(seed, J, row, k, P, lim, (u32)(j0 / 8 + b), buf.data() + ((size_t)i * ell + J) * T + 8 * b);
+    }
+  }
+  void begin(int i, int, const u64 *, int, int, int, int, const PrimeDev &) { cur = buf.data() + (size_t)i * ell * T; }
+  u64x2 c1(int J, int j) const { return ld2(cur + (size_t)J * T + (j - j0)); }
+};
+// every (row mi, coefficient pair j) of an element body replayed serially; SEED: one tile fill per row and T coefficients, body(mi,
+// j, tile) with the filled tile (nullptr without SEED)
+template <bool SEED, class Body>
+void seeded_replay(const u64 *const *keys, int n, long long koff, const PrimeDev *primes, int ell, int k, int N, Body body) {
+  SeedTileHost tile;
+  for (int mi = 0; mi <= ell; mi++) {
+    const int row = mi == ell ? k - 1 : mi;
+    for (int j0 = 0; j0 < N; j0 += SeedTileHost::T) {
+      if (SEED) tile.fill(keys, n, koff, ell, row, k, (size_t)N, primes[row], j0);
+      for (int j = j0; j < j0 + SeedTileHost::T && j < N; j += 2) body(mi, j, SEED ? &tile : nullptr);
+    }
+  }
+}
+template <int NOUT> void rot_wsum_ip_replay(const WsumIpArgs &A, long long koff, bool inl, bool seeded) {
+  if (seeded)
+    seeded_replay<true>(A.key, A.n, koff, A.primes, A.ell, A.k, A.N,
+                        [&](int mi, int j, SeedTileHost *t) { rot_wsum_ip_elem<NOUT, true, true>(A, mi, j, 0, koff, t); });
+  else
+    seeded_replay<false>(A.key, A.n, koff, A.primes, A.ell, A.k, A.N, [&](int mi, int j, SeedTileHost *) {
       if (inl) rot_wsum_ip_elem<NOUT, true>(A, mi, j, 0, koff);
       else rot_wsum_ip_elem<NOUT>(A, mi, j, 0, koff);
-    }
+    });
 }
 #endif
 // the inner products with the weighting: k_rot_wsum_ip in the CUDA build; compiled without CUDA (the CPU emulator of the tests) the
@@ -405,12 +461,12 @@ template <class BE> int rot_wsum_ip_step(BE &be, const WsumIpArgs &A) {
   return be.rot_wsum_ip(A);
 #else
   const long long koff = replay_key_off(be, 0);
-  const bool inl = hoist_inline_of(be, 0);
+  const bool inl = hoist_inline_of(be, 0), seeded = key_seeded_of(be, 0);   // seeded: inline (require_seeded_inline)
   switch (A.nout) {
-    case 1: rot_wsum_ip_replay<1>(A, koff, inl); break;
-    case 2: rot_wsum_ip_replay<2>(A, koff, inl); break;
-    case 3: rot_wsum_ip_replay<3>(A, koff, inl); break;
-    case 4: rot_wsum_ip_replay<4>(A, koff, inl); break;
+    case 1: rot_wsum_ip_replay<1>(A, koff, inl, seeded); break;
+    case 2: rot_wsum_ip_replay<2>(A, koff, inl, seeded); break;
+    case 3: rot_wsum_ip_replay<3>(A, koff, inl, seeded); break;
+    case 4: rot_wsum_ip_replay<4>(A, koff, inl, seeded); break;
     default: return be.error("rotate_wsum: 1..4 output sums");
   }
   return 0;
@@ -424,6 +480,7 @@ int rotate_wsum_impl(BE &be, const CtxView &c, int ell, int nout, u64 *out, cons
   if (n < 1 || n > WS_MAX) return be.error("rotate_wsum: 1..16 rotations");
   if (nout < 1 || nout > WS_OUT) return be.error("rotate_wsum: 1..4 output sums");
   if (ntap < 0 || ntap > WS_TAPS) return be.error("rotate_wsum: 0..16 plain taps");
+  if (int rc = require_seeded_inline(be)) return rc;
   const long long N = (long long)c.N;
   u64 *prow = work, *tmp = prow + (size_t)n * 2 * N;
   u64 *A = tmp + (size_t)n * 2 * N, *D = A + (size_t)nout * 2 * ell * N;
@@ -507,6 +564,7 @@ template <class BE>
 int lazy_rotsum_impl(BE &be, const CtxView &c, int ell, int nout, u64 *out, const u64 *a, const u64 *ext, int n, const u32 *const *perms,
                      const u64 *const *keys, const u64 *const *cadds, const u64 *const *wts, u64 *work) {
   if (hoist_inline_of(be, 0)) return be.error("lazy_rotsum (approx_hoist) takes stored hoist constants: turn evab_set_hoist_inline off");
+  if (key_seeded_of(be, 0)) return be.error("lazy_rotsum (approx_hoist) reads expanded keys: turn evab_set_key_seeded off");
   if (ell < 1 || ell > c.k - 1) return be.error("lazy_rotsum needs 1 <= ell <= k-1");
   if (n < 1 || n > LRS_MAX) return be.error("lazy_rotsum: 1..16 rotations");
   if (nout < 1 || nout > LRS_OUT) return be.error("lazy_rotsum: 1..4 output sums");

@@ -4,6 +4,7 @@
 // the CPU emulator.  Semantics: SURVEY.md Appendix A.4 / A.5 / A.8.
 #pragma once
 #include "ntt_core.cuh"
+#include "key_expand.cuh"
 
 enum { DY_ADD = 0, DY_SUB = 1, DY_NEG = 2, DY_MULPT = 3, DY_COPY = 4 };
 
@@ -186,12 +187,87 @@ EVAB_HD void inline_const(const u64 *ind, int row, size_t N, int j, const PrimeD
   c1.x = mulmod_p(reduce128(l1x, h1x, P), ni.x, P); c1.y = mulmod_p(reduce128(l1y, h1y, P), ni.y, P);
 }
 
+// ---- seeded key images (SEED = true; evab_set_key_seeded): the key operand of a key switch points at an image
+//   [k-1][k][N] c0 rows, then the key's 32-byte seed padded to 64 bytes      (seeded_key_words)
+// and its c1 rows -- the uniform half a, rows J k + m of the rule of key_expand.cuh -- are drawn where the expanded key's words are
+// loaded.  The key-bank offset moves the image, seed included.  A thread owns 2 coefficients and a ChaCha block yields 8, so the
+// draw is split from the inner product: a block (or the CPU replay) first draws the c1 words of its coefficient tile for every
+// J < ell of its row (seeded_c1_draw8 per ChaCha block, SeedTileDev / SeedTileHost), then the unchanged body reads them from that
+// tile (tile->c1).  The accepted candidates are reduced by barrett64 (exact for any 64-bit input), the rule's value.
+struct KxBarrett {
+  PrimeDev P;
+  EVAB_HD u64 operator()(u64 v) const { return barrett64(v, P.p, P.ratio64); }
+};
+EVAB_HD size_t seeded_key_words(int k, size_t N) { return (size_t)(k - 1) * k * N + 8; }
+// the c0 row (J, row) of a seeded image
+EVAB_HD const u64 *seeded_c0(const u64 *key, int J, int row, int k, size_t N) { return key + ((size_t)J * k + row) * N; }
+// coefficients 8 t .. 8 t + 7 of the c1 row (J, row) of the seeded image `key` (modulus P, lim = kx_limit(P.p)) -> dst
+EVAB_HD void seeded_c1_draw8(const uint32_t *seed, int J, int row, int k, const PrimeDev &P, u64 lim, u32 t, u64 *dst) {
+  u64 v[8];
+  kx_draw8(seed, (u64)J * k + row, t, KxBarrett{P}, lim, v);
+  // In a shared-memory tile, neighbouring lanes' blocks start 64 bytes apart, so each of these four 16-byte stores meets 4-way bank
+  // conflicts.  A lane-rotated store order that avoids them (selects on the lane) was measured slower by 1-3 % on every resident
+  // workload (DESIGN §4): the draw's ~1000 ALU instructions per block dominate, the selects cost more than the conflicts
+  kx_store8(dst, v);
+}
+EVAB_HD void seeded_seed(const u64 *key, int k, size_t N, uint32_t (&seed)[8]) {
+  const uint32_t *s = reinterpret_cast<const uint32_t *>(key + (size_t)(k - 1) * k * N);
+#pragma unroll
+  for (int i = 0; i < 8; i++) seed[i] = s[i];
+}
+// expanded keys: no tile (never dereferenced)
+struct SeedTileNone {
+  EVAB_HD void begin(int, int, const u64 *, int, int, int, int, const PrimeDev &) {}
+  EVAB_HD u64x2 c1(int, int) const { return u64x2{0, 0}; }
+};
+// the key words k0 = key[J][0][row], k1 = key[J][1][row] at coefficients j, j+1 of an expanded key, or of a seeded image and its tile
+template <bool SEED, class Tile> EVAB_HD void key_words(const u64 *key, const Tile *tile, int J, int row, int k, size_t N, int j, u64x2 &k0, u64x2 &k1) {
+  if (SEED) {
+    k0 = ld2(seeded_c0(key, J, row, k, N) + j);
+    k1 = tile->c1(J, j);
+  } else {
+    k0 = ld2(key + (((size_t)J * 2 + 0) * k + row) * N + j);
+    k1 = ld2(key + (((size_t)J * 2 + 1) * k + row) * N + j);
+  }
+}
+#if defined(__CUDACC__)
+// the tile of one thread block in shared memory: [ell][2 blockDim.x] words, coefficients j0 .. j0 + 2 blockDim.x - 1 of the block's
+// row, j0 = j - 2 threadIdx.x.  begin(i, j, ...) is called by every thread of the block with the same key and row (the kernels' tile
+// loops are uniform, N a multiple of the tile): a barrier (the previous tile's readers), ell / 4 ChaCha blocks per thread (rounded
+// up), a barrier
+struct SeedTileDev {
+  u64 *s;
+  EVAB_HD void begin(int, int j, const u64 *key, int ell, int row, int k, int N, const PrimeDev &P) {
+#if defined(__CUDA_ARCH__)
+    const int T = 2 * blockDim.x, per = T / 8;
+    const u32 t0 = (u32)(j - 2 * (int)threadIdx.x) / 8;
+    uint32_t seed[8];
+    seeded_seed(key, k, N, seed);
+    const u64 lim = kx_limit(P.p);
+    __syncthreads();
+    for (int b = threadIdx.x; b < ell * per; b += blockDim.x) seeded_c1_draw8(seed, b / per, row, k, P, lim, t0 + b % per, s + (size_t)(b / per) * T + (b % per) * 8);
+    __syncthreads();
+#endif
+  }
+  EVAB_HD u64x2 c1(int J, int) const {
+#if defined(__CUDA_ARCH__)
+    return ld2(s + (size_t)J * 2 * blockDim.x + 2 * threadIdx.x);
+#else
+    return u64x2{0, 0};
+#endif
+  }
+};
+#endif
+
 // off: batch instance offset (words) of t / ext / acc; koff: key offset (words) of the instance's tenant in a key bank
-// (evab_set_key_bank), applied to key and (INL = false) cadd; 0 when all instances share the key
-template <bool INL = false> EVAB_HD void ks_inner_elem(const IpArgs &A, int mi, int j, long long off = 0, long long koff = 0) {
+// (evab_set_key_bank), applied to key and (INL = false) cadd; 0 when all instances share the key.  SEED: key is a seeded image, its
+// c1 words come from `tile` (seeded_c1_draw8)
+template <bool INL = false, bool SEED = false, class Tile = SeedTileNone>
+EVAB_HD void ks_inner_elem(const IpArgs &A, int mi, int j, long long off = 0, long long koff = 0, Tile *tile = nullptr) {
   const int row = (mi == A.ell) ? A.k - 1 : mi;
   const PrimeDev P = A.primes[row];
   const size_t N = A.N;
+  if (SEED) tile->begin(0, j, A.key + koff, A.ell, row, A.k, A.N, P);
   u64 l0x = 0, h0x = 0, l0y = 0, h0y = 0, l1x = 0, h1x = 0, l1y = 0, h1y = 0;
   u64 s0x = 0, t0x = 0, s0y = 0, t0y = 0, s1x = 0, t1x = 0, s1y = 0, t1y = 0;   // INL: S_0, S_1
   for (int J = 0; J < A.ell; J++) {
@@ -205,8 +281,8 @@ template <bool INL = false> EVAB_HD void ks_inner_elem(const IpArgs &A, int mi, 
       if (A.eperm) { v.x = EVAB_LDG(ep + EVAB_LDG(A.eperm + j)); v.y = EVAB_LDG(ep + EVAB_LDG(A.eperm + j + 1)); }
       else v = ld2(ep + j);
     }
-    const u64x2 k0 = ld2(A.key + koff + (((size_t)J * 2 + 0) * A.k + row) * N + j);
-    const u64x2 k1 = ld2(A.key + koff + (((size_t)J * 2 + 1) * A.k + row) * N + j);
+    u64x2 k0, k1;
+    key_words<SEED>(A.key + koff, tile, J, row, A.k, N, j, k0, k1);
     mac128(l0x, h0x, v.x, k0.x); mac128(l0y, h0y, v.y, k0.y);
     mac128(l1x, h1x, v.x, k1.x); mac128(l1y, h1y, v.y, k1.y);
     if (INL && J != row) {
@@ -250,19 +326,21 @@ struct RotManyArgs {
   int n, ell, k, N;
 };
 // koff: key offset of the instance's tenant (ks_inner_elem), applied to key[i] and (INL = false) cadd[i]; INL: cadd[i] is the
-// element's indicator rows (ks_inner_elem)
-template <bool INL = false> EVAB_HD void rot_many_elem(const RotManyArgs &A, int i, int mi, int j, long long off = 0, long long koff = 0) {
+// element's indicator rows (ks_inner_elem); SEED: key[i] is a seeded image (ks_inner_elem)
+template <bool INL = false, bool SEED = false, class Tile = SeedTileNone>
+EVAB_HD void rot_many_elem(const RotManyArgs &A, int i, int mi, int j, long long off = 0, long long koff = 0, Tile *tile = nullptr) {
   const int row = (mi == A.ell) ? A.k - 1 : mi;
   const PrimeDev P = A.primes[row];
   const size_t N = A.N;
+  if (SEED) tile->begin(i, j, A.key[i] + koff, A.ell, row, A.k, A.N, P);
   const u32 pj0 = EVAB_LDG(A.perm[i] + j), pj1 = EVAB_LDG(A.perm[i] + j + 1);
   u64 l0x = 0, h0x = 0, l0y = 0, h0y = 0, l1x = 0, h1x = 0, l1y = 0, h1y = 0;
   u64 s0x = 0, t0x = 0, s0y = 0, t0y = 0, s1x = 0, t1x = 0, s1y = 0, t1y = 0;   // INL: S_0, S_1
   for (int J = 0; J < A.ell; J++) {
     const u64 *src = (row == J) ? A.t + off + (size_t)J * N : A.ext + off + ((size_t)mi * A.ell + J) * N;
     const u64 vx = EVAB_LDG(src + pj0), vy = EVAB_LDG(src + pj1);
-    const u64x2 k0 = ld2(A.key[i] + koff + (((size_t)J * 2 + 0) * A.k + row) * N + j);
-    const u64x2 k1 = ld2(A.key[i] + koff + (((size_t)J * 2 + 1) * A.k + row) * N + j);
+    u64x2 k0, k1;
+    key_words<SEED>(A.key[i] + koff, tile, J, row, A.k, N, j, k0, k1);
     mac128(l0x, h0x, vx, k0.x); mac128(l0y, h0y, vy, k0.y);
     mac128(l1x, h1x, vx, k1.x); mac128(l1y, h1y, vy, k1.y);
     if (INL && J != row) {
@@ -387,8 +465,9 @@ struct WsumIpArgs {
 // rot_many_elem's canonical value: the inner product through perm_i + cadd_i, and on a q row + perm_i(P c0) = (P mod q_m) c0[perm_i(j)],
 // read from c0 directly.  A P row is stored; a q row is weighted into A, which then takes the taps.
 // koff: key offset of the instance's tenant (ks_inner_elem), applied to key[i] and (INL = false) cadd[i]; INL: cadd[i] is the
-// element's indicator rows (ks_inner_elem)
-template <int NOUT, bool INL = false> EVAB_HD void rot_wsum_ip_elem(const WsumIpArgs &A, int mi, int j, long long off = 0, long long koff = 0) {
+// element's indicator rows (ks_inner_elem); SEED: key[i] is a seeded image, and every rotation begins its own tile (ks_inner_elem)
+template <int NOUT, bool INL = false, bool SEED = false, class Tile = SeedTileNone>
+EVAB_HD void rot_wsum_ip_elem(const WsumIpArgs &A, int mi, int j, long long off = 0, long long koff = 0, Tile *tile = nullptr) {
   const bool qrow = mi < A.ell;
   const int row = qrow ? mi : A.k - 1;
   const PrimeDev P = A.primes[row];
@@ -406,11 +485,12 @@ template <int NOUT, bool INL = false> EVAB_HD void rot_wsum_ip_elem(const WsumIp
     if (i + 1 < A.n) { pj0 = EVAB_LDG(A.perm[i + 1] + j); pj1 = EVAB_LDG(A.perm[i + 1] + j + 1); }   // the next gather's addresses
     u64 l0x = 0, h0x = 0, l0y = 0, h0y = 0, l1x = 0, h1x = 0, l1y = 0, h1y = 0;
     u64 s0x = 0, t0x = 0, s0y = 0, t0y = 0, s1x = 0, t1x = 0, s1y = 0, t1y = 0;   // INL: S_0, S_1
+    if (SEED) tile->begin(i, j, A.key[i] + koff, A.ell, row, A.k, A.N, P);
     for (int J = 0; J < A.ell; J++) {
       const u64 *src = (row == J) ? A.t + off + (size_t)J * N : A.ext + off + ((size_t)mi * A.ell + J) * N;
       const u64 vx = EVAB_LDG(src + p0), vy = EVAB_LDG(src + p1);
-      const u64x2 k0 = ld2(A.key[i] + koff + (((size_t)J * 2 + 0) * A.k + row) * N + j);
-      const u64x2 k1 = ld2(A.key[i] + koff + (((size_t)J * 2 + 1) * A.k + row) * N + j);
+      u64x2 k0, k1;
+      key_words<SEED>(A.key[i] + koff, tile, J, row, A.k, N, j, k0, k1);
       mac128(l0x, h0x, vx, k0.x); mac128(l0y, h0y, vy, k0.y);
       mac128(l1x, h1x, vx, k1.x); mac128(l1y, h1y, vy, k1.y);
       if (INL && J != row) {

@@ -100,6 +100,15 @@ int evab_set_key_bank(const int32_t *d_tenant_of_instance, size_t tenant_stride_
  * from the key rows it loads (same bits); those rows are shared by all tenants of a key bank and are NOT shifted by the
  * key-bank offset.  evab_lazy_rotsum fails while it is on. */
 int evab_set_hoist_inline(int on);
+/* Seeded keys, thread-local like evab_set_key_bank (on != 0: on).  While on, the d_key / d_keys[i] arguments of
+ * evab_relinearize, evab_rotate, evab_rotate_prepared, evab_rotate_modup_prepared, evab_rotate_modup_many and evab_rotate_wsum
+ * point at seeded key images of evab_seeded_key_bytes bytes: the key's [k-1][k][N] c0 rows, then its 32-byte seed padded to 64
+ * bytes.  The c1 rows are never stored: the key-switch inner products draw them from the seed by the rule of
+ * eva_b200/csrc/key_expand.cuh (the words evab_expand_key_uniform writes), so the outputs are those of the expanded key.  The
+ * key-bank offset moves the whole image.  The hoisted calls need evab_set_hoist_inline on; evab_lazy_rotsum,
+ * evab_rotate_hoist_const and evab_rotate_hoist_const_levels fail while it is on. */
+int evab_set_key_seeded(int on);
+size_t evab_seeded_key_bytes(const evab_ctx *ctx);
 /* number of kernel launches issued through this context so far */
 uint64_t evab_launch_count(const evab_ctx *ctx);
 
