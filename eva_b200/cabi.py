@@ -92,6 +92,8 @@ _SIGS = {
     "evab_set_hoist_inline": (ci, [ci]),
     "evab_set_key_seeded": (ci, [ci]),
     "evab_seeded_key_bytes": (szt, [vp]),
+    "evab_set_key_c1_rows": (ci, [vp]),
+    "evab_expand_seeded_c1": (ci, [vp, ci, vp, vp, vp]),
     "evab_mod_switch": (ci, [vp, ci, vp, vp, ci, vp]),
     "evab_keyswitch_work_bytes": (szt, [vp, ci]),
     "evab_relinearize": (ci, [vp, ci, vp, vp, vp, vp, vp]),

@@ -59,11 +59,18 @@ extern "C" int evab_set_batch(int batch, size_t stride_words, size_t value_strid
   return 0;
 }
 // thread-local key selection (evab_set_key_bank): instance b reads its keys at + tenant[b] * stride words
-struct KeyBankSel { const int32_t *tenant = nullptr; long long stride = 0; };
+// c1: the c1 region of every instance (evab_set_key_c1_rows), read by the C1 instances only
+struct KeyBankSel { const int32_t *tenant = nullptr; long long stride = 0; const int32_t *c1 = nullptr; };
 static thread_local KeyBankSel g_bank;
 extern "C" int evab_set_key_bank(const int32_t *d_tenant_of_instance, size_t tenant_stride_words) {
   g_bank.tenant = d_tenant_of_instance;
   g_bank.stride = d_tenant_of_instance ? (long long)tenant_stride_words : 0;
+  return 0;
+}
+// thread-local cached c1 rows (evab_set_key_c1_rows): instance b of a seeded bank launch reads its keys' c1 rows at + region[b] *
+// stride words, or draws them (region[b] < 0)
+extern "C" int evab_set_key_c1_rows(const int32_t *d_region_of_instance) {
+  g_bank.c1 = d_region_of_instance;
   return 0;
 }
 // thread-local inline hoist constants (evab_set_hoist_inline): the cadd operands of the hoisted rotations are indicator rows
@@ -220,17 +227,25 @@ __global__ void __launch_bounds__(256) k_sum_terms(const SumArgs A, const long l
 }
 // key offset of this block's instance: BANK = false is the shared-key launch (offset 0, the table is not read)
 template <bool BANK> __device__ __forceinline__ long long key_off(const KeyBankSel &K) { return BANK ? (long long)__ldg(K.tenant + blockIdx.z) * K.stride : 0; }
-// SEED: the c1 tile of a seeded key, [ell][2 blockDim.x] words of dynamic shared memory (seed_tile_bytes; ops_kernels.cuh SeedTileDev)
-__device__ __forceinline__ SeedTileDev seed_tile() {
+// SEED: the c1 tile of a seeded key, [ell][2 blockDim.x] words of dynamic shared memory (seed_tile_bytes; ops_kernels.cuh SeedTileDev).
+// C1 (seeded bank launches with evab_set_key_c1_rows): the block's instance copies its c1 rows from region K.c1[blockIdx.z] when it
+// has one; the tile's offset is taken from the tenant's image (key + koff) to the region (key + region * stride)
+template <bool C1 = false> __device__ __forceinline__ SeedTileDev seed_tile(const KeyBankSel &K, long long koff) {
   extern __shared__ __align__(16) u64 sm[];
-  return SeedTileDev{sm};
+  SeedTileDev t{sm};
+  if (C1) {
+    const int r = __ldg(K.c1 + blockIdx.z);
+    t.cached = r >= 0;
+    t.c1d = (long long)r * K.stride - koff;
+  }
+  return t;
 }
 // INL: inline hoist constants (ks_inner_elem); SEED: seeded key images (every launch has N / 512 blocks per row or a multiple of
 // them, so the tile loop is uniform over the block)
-template <bool BANK, bool INL, bool SEED> __global__ void __launch_bounds__(256) k_ks_inner(const IpArgs A, const long long bstride, const KeyBankSel K) {
+template <bool BANK, bool INL, bool SEED, bool C1 = false> __global__ void __launch_bounds__(256) k_ks_inner(const IpArgs A, const long long bstride, const KeyBankSel K) {
   const long long off = (long long)blockIdx.z * bstride;   // parameters stay in constant memory: no local copy
   const long long koff = key_off<BANK>(K);
-  SeedTileDev tile = seed_tile();
+  SeedTileDev tile = seed_tile<C1>(K, koff);
   for (int j = (blockIdx.x * blockDim.x + threadIdx.x) * 2; j < A.N; j += gridDim.x * blockDim.x * 2)
     ks_inner_elem<INL, SEED>(A, blockIdx.y, j, off, koff, SEED ? &tile : nullptr);
 }
@@ -239,17 +254,17 @@ __global__ void __launch_bounds__(256) k_scale_c0(const u64 *c0, u64 *ext, const
   for (int j = blockIdx.x * blockDim.x + threadIdx.x; j < N; j += gridDim.x * blockDim.x) scale_c0_elem(c0, ext, primes, ell, k, N, blockIdx.y, j, off);
 }
 // INL: 3 blocks per SM (80 registers) -- at 4 the inline instance spills about 100 bytes
-template <bool BANK, bool INL, bool SEED> __global__ void __launch_bounds__(256, INL ? 3 : 4) k_rot_many(const RotManyArgs A, const long long bstride, const KeyBankSel K) {
+template <bool BANK, bool INL, bool SEED, bool C1 = false> __global__ void __launch_bounds__(256, INL ? 3 : 4) k_rot_many(const RotManyArgs A, const long long bstride, const KeyBankSel K) {
   const long long off = (long long)blockIdx.z * bstride, koff = key_off<BANK>(K);
   const int i = blockIdx.y / (A.ell + 1), mi = blockIdx.y % (A.ell + 1);
-  SeedTileDev tile = seed_tile();
+  SeedTileDev tile = seed_tile<C1>(K, koff);
   for (int j = (blockIdx.x * blockDim.x + threadIdx.x) * 2; j < A.N; j += gridDim.x * blockDim.x * 2)
     rot_many_elem<INL, SEED>(A, i, mi, j, off, koff, SEED ? &tile : nullptr);
 }
 // grid.y = row of the extended basis; every thread loops over the rotations, so blocks are kept small for more of them
-template <int NOUT, bool BANK, bool INL, bool SEED> __global__ void __launch_bounds__(128) k_rot_wsum_ip(const WsumIpArgs A, const long long bstride, const KeyBankSel K) {
+template <int NOUT, bool BANK, bool INL, bool SEED, bool C1 = false> __global__ void __launch_bounds__(128) k_rot_wsum_ip(const WsumIpArgs A, const long long bstride, const KeyBankSel K) {
   const long long off = (long long)blockIdx.z * bstride, koff = key_off<BANK>(K);
-  SeedTileDev tile = seed_tile();
+  SeedTileDev tile = seed_tile<C1>(K, koff);
   for (int j = (blockIdx.x * blockDim.x + threadIdx.x) * 2; j < A.N; j += gridDim.x * blockDim.x * 2)
     rot_wsum_ip_elem<NOUT, INL, SEED>(A, blockIdx.y, j, off, koff, SEED ? &tile : nullptr);
 }
@@ -292,6 +307,11 @@ __global__ void __launch_bounds__(256) k_hoist_const_levels(const HoistLevelsArg
 __global__ void __launch_bounds__(256) k_expand_uniform(const ExpandArgs A) {
   const u32 t = blockIdx.x * blockDim.x + threadIdx.x;
   if (t < A.N / 8) expand_uniform_elem(A, blockIdx.z, blockIdx.y, t);
+}
+// grid (blocks of 8 coefficients, c1 row r, seeded image i): one ChaCha20 block per thread
+__global__ void __launch_bounds__(256) k_expand_seeded_c1(const u64 *images, u64 *rows, const PrimeDev *primes, int k, int N) {
+  const u32 t = blockIdx.x * blockDim.x + threadIdx.x;
+  if (t < (u32)N / 8) expand_seeded_c1_elem(images, rows, primes, k, (size_t)N, blockIdx.z, blockIdx.y, t);
 }
 // grid (blocks of 8 coefficients, ciphertext row m, entry i of the launch): one ChaCha20 block per thread; rows m >= ell_i return
 __global__ void __launch_bounds__(256) k_expand_cipher_uniform(const CipherExpandArgs A) {
@@ -450,7 +470,9 @@ static int seeded_smem_opt_in(int k) {
   const size_t b = seed_tile_bytes(k - 1, 256);
   if (seed_smem_allow(k_ks_inner<false, false, true>, b) || seed_smem_allow(k_ks_inner<false, true, true>, b) ||
       seed_smem_allow(k_ks_inner<true, false, true>, b) || seed_smem_allow(k_ks_inner<true, true, true>, b) ||
-      seed_smem_allow(k_rot_many<false, true, true>, b) || seed_smem_allow(k_rot_many<true, true, true>, b))
+      seed_smem_allow(k_rot_many<false, true, true>, b) || seed_smem_allow(k_rot_many<true, true, true>, b) ||
+      seed_smem_allow(k_ks_inner<true, false, true, true>, b) || seed_smem_allow(k_ks_inner<true, true, true, true>, b) ||
+      seed_smem_allow(k_rot_many<true, true, true, true>, b))
     return 1;
   static_assert(24 * 2 * 128 * sizeof(u64) <= 48 * 1024, "the k_rot_wsum_ip seeded tile fits the default shared memory");
   return 0;
@@ -462,6 +484,9 @@ struct CudaBE {
   int error(const char *m) { return fail(m); }
   bool hoist_inline() const { return g_inline; }
   bool key_seeded() const { return g_seeded; }
+  bool key_bank() const { return g_bank.tenant != nullptr; }
+  // cached c1 rows: checked by require_c1_rows (seeded keys and a key-bank table), so the C1 instances are bank instances only
+  bool key_c1_rows() const { return g_bank.c1 != nullptr; }
   // dynamic shared memory of a seeded launch (the c1 tile, SeedTileDev); the instances whose tile can pass the 48 KB default were
   // allowed their largest one when the context was created (seeded_smem_opt_in), so a launch -- or a graph capture -- sets nothing
   static size_t seed_smem(int ell, int threads) { return seed_tile_bytes(ell, threads); }
@@ -523,16 +548,17 @@ struct CudaBE {
     CUDA_OK(cudaGetLastError());
     return 0;
   }
-  template <bool BANK> void inner_seeded(dim3 g, const IpArgs &A, bool inl) {
-    if (inl) k_ks_inner<BANK, true, true><<<g, 256, seed_smem(A.ell, 256), st>>>(A, g_batch.stride, g_bank);
-    else k_ks_inner<BANK, false, true><<<g, 256, seed_smem(A.ell, 256), st>>>(A, g_batch.stride, g_bank);
+  template <bool BANK, bool C1 = false> void inner_seeded(dim3 g, const IpArgs &A, bool inl) {
+    if (inl) k_ks_inner<BANK, true, true, C1><<<g, 256, seed_smem(A.ell, 256), st>>>(A, g_batch.stride, g_bank);
+    else k_ks_inner<BANK, false, true, C1><<<g, 256, seed_smem(A.ell, 256), st>>>(A, g_batch.stride, g_bank);
   }
   int inner(const IpArgs &A) {
     count();
     const dim3 g = grid(A.ell + 1);
     const bool inl = g_inline && A.cadd;   // only the hoisted form has a constant to form
     if (g_seeded) {
-      if (g_bank.tenant) inner_seeded<true>(g, A, inl);
+      if (g_bank.c1) inner_seeded<true, true>(g, A, inl);
+      else if (g_bank.tenant) inner_seeded<true>(g, A, inl);
       else inner_seeded<false>(g, A, inl);
     }
     else if (g_bank.tenant) { if (inl) k_ks_inner<true, true, false><<<g, 256, 0, st>>>(A, g_batch.stride, g_bank); else k_ks_inner<true, false, false><<<g, 256, 0, st>>>(A, g_batch.stride, g_bank); }
@@ -551,7 +577,8 @@ struct CudaBE {
     count();
     const dim3 g = grid(A.n * (A.ell + 1));
     if (g_seeded) {   // inline constants (require_seeded_inline)
-      if (g_bank.tenant) k_rot_many<true, true, true><<<g, 256, seed_smem(A.ell, 256), st>>>(A, g_batch.stride, g_bank);
+      if (g_bank.c1) k_rot_many<true, true, true, true><<<g, 256, seed_smem(A.ell, 256), st>>>(A, g_batch.stride, g_bank);
+      else if (g_bank.tenant) k_rot_many<true, true, true><<<g, 256, seed_smem(A.ell, 256), st>>>(A, g_batch.stride, g_bank);
       else k_rot_many<false, true, true><<<g, 256, seed_smem(A.ell, 256), st>>>(A, g_batch.stride, g_bank);
     }
     else if (g_bank.tenant) { if (g_inline) k_rot_many<true, true, false><<<g, 256, 0, st>>>(A, g_batch.stride, g_bank); else k_rot_many<true, false, false><<<g, 256, 0, st>>>(A, g_batch.stride, g_bank); }
@@ -562,7 +589,8 @@ struct CudaBE {
   }
   template <int NOUT> void wsum_ip(dim3 g, const WsumIpArgs &A, bool bank) {
     if (g_seeded) {   // inline constants (require_seeded_inline)
-      if (bank) k_rot_wsum_ip<NOUT, true, true, true><<<g, 128, seed_smem(A.ell, 128), st>>>(A, g_batch.stride, g_bank);
+      if (g_bank.c1) k_rot_wsum_ip<NOUT, true, true, true, true><<<g, 128, seed_smem(A.ell, 128), st>>>(A, g_batch.stride, g_bank);
+      else if (bank) k_rot_wsum_ip<NOUT, true, true, true><<<g, 128, seed_smem(A.ell, 128), st>>>(A, g_batch.stride, g_bank);
       else k_rot_wsum_ip<NOUT, false, true, true><<<g, 128, seed_smem(A.ell, 128), st>>>(A, g_batch.stride, g_bank);
     }
     else if (bank) { if (g_inline) k_rot_wsum_ip<NOUT, true, true, false><<<g, 128, 0, st>>>(A, g_batch.stride, g_bank); else k_rot_wsum_ip<NOUT, true, false, false><<<g, 128, 0, st>>>(A, g_batch.stride, g_bank); }
@@ -1070,6 +1098,18 @@ extern "C" int evab_expand_key_uniform(evab_ctx *c, int n, const uint8_t *seeds,
   CUDA_OK(cudaSetDevice(c->device));
   c->launches.fetch_add(1, std::memory_order_relaxed);
   k_expand_uniform<<<dim3((A.N / 8 + 255) / 256, (A.k - 1) * A.k, n), 256, 0, S(stream)>>>(A);
+  CUDA_OK(cudaGetLastError());
+  return 0;
+}
+extern "C" int evab_expand_seeded_c1(evab_ctx *c, int n, const uint64_t *images, uint64_t *rows, void *stream) {
+  if (n < 1 || n > 65535) return fail("evab_expand_seeded_c1: n must be in [1, 65535]");
+  if (!images || !rows) return fail("evab_expand_seeded_c1: d_images and d_rows must not be null");
+  if (c->v.k < 2) return fail("evab_expand_seeded_c1: seeded keys need k >= 2 primes");
+  if (reinterpret_cast<uintptr_t>(images) % 64 || reinterpret_cast<uintptr_t>(rows) % 64)
+    return fail("evab_expand_seeded_c1: d_images and d_rows must be 64-byte aligned");
+  CUDA_OK(cudaSetDevice(c->device));
+  c->launches.fetch_add(1, std::memory_order_relaxed);
+  k_expand_seeded_c1<<<dim3(((unsigned)c->v.N / 8 + 255) / 256, (c->v.k - 1) * c->v.k, n), 256, 0, S(stream)>>>(images, rows, c->v.primes, c->v.k, (int)c->v.N);
   CUDA_OK(cudaGetLastError());
   return 0;
 }

@@ -148,6 +148,8 @@ public:
     }
   }
   const SlotCache &cache() const { return cache_; }
+  // the event of the last fill of a slot (null: never filled by the pager)
+  void *fillEvent(int slot) const { return fillEv_[slot]; }
   std::size_t hostBytes() const {
     std::size_t w = 0;
     for (const Block &b : host_) w += b.words;
@@ -176,16 +178,83 @@ private:
   void *stream_ = nullptr;                          // fills
 };
 
+// Cached c1 rows of a seeded key bank (B200Server c1_cache): C1Cache decides which tenants hold the bank's c1 regions, and a fill
+// expands a tenant's c1 rows from the seeds in its bank slot (KeyBank::fillC1) on the store's own stream.  A fill waits for the
+// fill of the tenant's slot (paging: its images must be there) and for the runs that may still read the region (one reader event
+// per region and replica stream), and records the region's fill event, which every run that reads the region waits for.  The rows
+// depend on the seeds only, so a tenant keeps its region while its slot is paged out and back in; removing its keys drops it.
+class C1Store {
+public:
+  C1Store(std::shared_ptr<Device> dev, KeyBank &bank, KeyPager *pager)
+      : dev_(std::move(dev)), bank_(bank), pager_(pager), cache_(bank.c1Regions()), fillEv_(bank.c1Regions(), nullptr), readers_(bank.c1Regions()) {
+    check(evab_stream_create(dev_->ctx(), &stream_));
+  }
+  ~C1Store() {
+    evab_ctx *c = dev_->ctx();
+    evab_sync(c, stream_);
+    for (void *e : fillEv_) if (e) evab_event_destroy(c, e);
+    for (auto &m : readers_) for (auto &r : m) evab_event_destroy(c, r.second);
+    evab_stream_destroy(c, stream_);
+  }
+  C1Store(const C1Store &) = delete;
+  // the c1 table entry of every instance of a batch (bank region capacity + h, or -1: draws) whose instances hold bank slots
+  // `slots`; the admitted missing tenants' fills are enqueued on the store's stream
+  std::vector<int> resolve(const std::vector<int> &tenants, const std::vector<int> &slots) {
+    evab_ctx *c = dev_->ctx();
+    std::vector<C1Cache::Fill> fills;
+    std::vector<int> regions = cache_.assign(tenants, fills);
+    for (auto &f : fills) {
+      const int slot = slots[std::find(tenants.begin(), tenants.end(), f.tenant) - tenants.begin()];
+      for (auto &r : readers_[f.region]) check(evab_stream_wait_event(c, stream_, r.second));
+      if (pager_) if (void *ev = pager_->fillEvent(slot)) check(evab_stream_wait_event(c, stream_, ev));
+      bank_.fillC1(f.region, slot, stream_);
+      if (!fillEv_[f.region]) check(evab_event_create(c, &fillEv_[f.region]));
+      check(evab_event_record(c, fillEv_[f.region], stream_));
+    }
+    for (int &r : regions) if (r >= 0) r += bank_.capacity();
+    return regions;
+  }
+  // a run on `stream` with c1 table entries `rows` waits for their regions' fills; once enqueued, it is recorded as their reader
+  void beforeRun(void *stream, const int *rows, int n) {
+    for (int i = 0; i < n; i++)
+      if (rows[i] >= 0 && std::find(rows, rows + i, rows[i]) == rows + i) {
+        if (void *ev = fillEv_[rows[i] - bank_.capacity()]) check(evab_stream_wait_event(dev_->ctx(), stream, ev));
+      }
+  }
+  void afterRun(void *stream, const int *rows, int n) {
+    for (int i = 0; i < n; i++) {
+      if (rows[i] < 0 || std::find(rows, rows + i, rows[i]) != rows + i) continue;
+      void *&ev = readers_[rows[i] - bank_.capacity()][stream];
+      if (!ev) check(evab_event_create(dev_->ctx(), &ev));
+      check(evab_event_record(dev_->ctx(), ev, stream));
+    }
+  }
+  void drop(int tenant) { cache_.drop(tenant); }
+  const C1Cache &cache() const { return cache_; }
+
+private:
+  std::shared_ptr<Device> dev_;
+  KeyBank &bank_;
+  KeyPager *pager_;
+  C1Cache cache_;
+  std::vector<void *> fillEv_;                      // region -> event of its last fill
+  std::vector<std::map<void *, void *>> readers_;   // region -> (replica stream -> event after its last run that read the region)
+  void *stream_ = nullptr;                          // fills
+};
+
 struct Shared {
   std::shared_ptr<Device> dev;
   std::unique_ptr<CkksClient> client;
   KeySet keys;
   std::unique_ptr<KeyBank> bank;   // B200Server: the tenants' keys (then `keys` is empty and every batch names a tenant per instance)
   std::unique_ptr<KeyPager> pager; // B200Server with max_tenants > capacity: tenants paged into the bank's regions
+  std::unique_ptr<C1Store> c1;     // B200Server with c1_cache > 0: cached c1 rows of a seeded bank (declared after pager: destroyed first)
   std::mutex execMutex;   // serialises execute / executeMany callers of one context (see executeMany), and key-bank changes
   void requireTenant(int t) const { if (pager) pager->requireRegistered(t); else bank->requireOccupied(t); }
   // the bank region of every instance (with paging: resolved, and missing tenants' fills enqueued)
   std::vector<int> slotsFor(const std::vector<int> &tenants) { return pager ? pager->resolve(tenants) : tenants; }
+  // the c1 table entry of every instance (with a c1 cache: resolved, and admitted tenants' fills enqueued; else empty)
+  std::vector<int> c1For(const std::vector<int> &tenants, const std::vector<int> &slots) { return c1 ? c1->resolve(tenants, slots) : std::vector<int>(); }
 };
 
 // SEALPublic::encrypt's checks, slot replication and encoding (reference eva/seal/seal.cpp:24-102), shared by the public-key
@@ -428,7 +497,9 @@ public:
     std::vector<char> busy(R, 0);
     // key-bank region of every instance, resolved at every enqueue (so that collect's redo refills a tenant evicted meanwhile)
     const std::vector<int> slots = p.tenants.empty() ? std::vector<int>() : s_->slotsFor(p.tenants);
+    const std::vector<int> c1 = p.tenants.empty() ? std::vector<int>() : s_->c1For(p.tenants, slots);
     KeyPager *pager = s_->pager.get();
+    C1Store *c1s = s_->c1.get();
     for (int b0 = 0, g = 0; b0 < B; b0 += F, g++) {
       const int nb = std::min(F, B - b0);
       const int r = g % R;
@@ -439,14 +510,17 @@ public:
       if (busy[r]) s_->dev->sync(st);   // the replica's arena is reused: wait for its previous chunk
       busy[r] = 1;
       if (!slots.empty()) ex.setTenants(slots.data() + b0, nb);
+      if (!c1.empty()) ex.setC1Rows(c1.data() + b0, nb);
       if (std::find(streams.begin(), streams.end(), st) == streams.end()) streams.push_back(st);
       if (std::find(p.plans.begin(), p.plans.end(), holder) == p.plans.end()) p.plans.push_back(holder);
       auto t1 = now();
       stageInputs(ex, program, inputs.data() + b0, nb, st);
       auto t2 = now();
       if (pager) pager->beforeRun(st, slots.data() + b0, nb);
+      if (c1s) c1s->beforeRun(st, c1.data() + b0, nb);
       ex.run(st);
       if (pager) pager->afterRun(st, slots.data() + b0, nb);
+      if (c1s) c1s->afterRun(st, c1.data() + b0, nb);
       auto t3 = now();
       tPlan += std::chrono::duration<double>(t1 - t0).count(); tStage += std::chrono::duration<double>(t2 - t1).count();
       tRun += std::chrono::duration<double>(t3 - t2).count();
@@ -496,15 +570,21 @@ public:
   // rotationKeys: the bank's Galois keys (rotationKeySteps); rotations without a key of their own are composed.
   // hoistConstants: "stored" -- every region holds the hoist constants of its keys; "inline" -- keys only, the constants are formed
   // inside the key-switch inner products (KeyBank).  keyStorage: "expanded" -- every key in full; "seeded" (inline constants only) --
-  // c0 rows and seeds, the key switches draw the c1 rows (KeyBank)
+  // c0 rows and seeds, the key switches draw the c1 rows (KeyBank).  c1Cache (seeded keys, 0 .. capacity): regions holding the
+  // expanded c1 rows of the tenants used most (C1Store); 0 is the plain seeded bank
   B200Server(const CKKSParameters &params, int capacity, int device, int maxTenants = -1, const std::string &rotationKeys = "program",
-             const std::string &hoistConstants = "stored", const std::string &keyStorage = "expanded")
+             const std::string &hoistConstants = "stored", const std::string &keyStorage = "expanded", int c1Cache = 0)
       : rotationKeys_(rotationKeys), hoistConstants_(hoistConstants), keyStorage_(keyStorage) {
     if (hoistConstants != "stored" && hoistConstants != "inline")
       throw std::invalid_argument("hoist_constants must be \"stored\" or \"inline\", not \"" + hoistConstants + "\"");
     if (keyStorage != "expanded" && !(keyStorage == "seeded" && hoistConstants == "inline"))
       throw std::invalid_argument("key_storage must be \"expanded\", or \"seeded\" with hoist_constants=\"inline\" (got key_storage=\"" +
                                   keyStorage + "\", hoist_constants=\"" + hoistConstants + "\")");
+    if (c1Cache < 0 || c1Cache > capacity)
+      throw std::invalid_argument("c1_cache (" + std::to_string(c1Cache) + ") must be in [0, capacity] (capacity " + std::to_string(capacity) + ")");
+    if (c1Cache > 0 && keyStorage != "seeded")
+      throw std::invalid_argument("c1_cache (" + std::to_string(c1Cache) + ") caches the c1 rows of seeded keys: it needs key_storage=\"seeded\" (got key_storage=\"" +
+                                  keyStorage + "\")");
     if (maxTenants >= 0 && maxTenants < capacity)
       throw std::invalid_argument("max_tenants (" + std::to_string(maxTenants) + ") is below the number of device slots (capacity " + std::to_string(capacity) + ")");
     const std::vector<int> steps = rotationKeySteps(params, rotationKeys);
@@ -518,8 +598,9 @@ public:
       if (!elt) throw std::invalid_argument("step count too large");
       elts.insert(elt);
     }
-    s->bank = std::make_unique<KeyBank>(s->dev, elts, capacity, hoistConstants == "inline", keyStorage == "seeded");
+    s->bank = std::make_unique<KeyBank>(s->dev, elts, capacity, hoistConstants == "inline", keyStorage == "seeded", c1Cache);
     if (maxTenants > capacity) s->pager = std::make_unique<KeyPager>(s->dev, *s->bank, maxTenants);
+    if (c1Cache > 0) s->c1 = std::make_unique<C1Store>(s->dev, *s->bank, s->pager.get());
     pub_ = std::make_unique<B200Public>(s);
   }
   // host images [k-1][2][k][N] (shapes checked by the caller); every element of the rotation set must be present
@@ -546,6 +627,7 @@ public:
     std::lock_guard<std::mutex> guard(shared()->execMutex);
     shared()->requireTenant(t);
     if (pub_->tenantInFlightLocked(t)) throw std::runtime_error("tenant " + std::to_string(t) + " is used by a batch that has not been collected");
+    if (shared()->c1) shared()->c1->drop(t);   // an id reused with new keys never reads this tenant's rows
     if (shared()->pager) shared()->pager->remove(t);
     else shared()->bank->remove(t);
   }
@@ -558,7 +640,8 @@ public:
     for (int t : tenants) shared()->requireTenant(t);
     Executor &ex = pub_->executorFor(prog, (int)rq.size(), replica);
     staged_[&ex] = tenants;
-    setSlots(ex, shared()->slotsFor(tenants), stream);
+    const std::vector<int> slots = shared()->slotsFor(tenants);
+    setSlots(ex, slots, shared()->c1For(tenants, slots), stream);
     std::vector<const B200Valuation *> in;
     for (auto &r : rq) in.push_back(r.second);
     pub_->stageInputs(ex, prog, in.data(), (int)in.size(), stream);
@@ -578,10 +661,13 @@ public:
     if (it == staged_.end()) throw std::runtime_error("run_resident: stage the replica's inputs first");
     if (pager) for (int t : it->second) pager->requireRegistered(t);
     const std::vector<int> slots = shared()->slotsFor(it->second);
-    setSlots(ex, slots, stream);
+    const std::vector<int> c1 = shared()->c1For(it->second, slots);
+    setSlots(ex, slots, c1, stream);
     if (pager) pager->beforeRun(stream, slots.data(), batch);
+    if (!c1.empty()) shared()->c1->beforeRun(stream, c1.data(), batch);
     ex.run(stream);
     if (pager) pager->afterRun(stream, slots.data(), batch);
+    if (!c1.empty()) shared()->c1->afterRun(stream, c1.data(), batch);
   }
   std::shared_ptr<PendingBatch> submit(Program &program, const std::vector<std::pair<int, const B200Valuation *>> &requests, int slot = 0) {
     std::vector<const B200Valuation *> in;
@@ -601,11 +687,13 @@ public:
   std::shared_ptr<Shared> shared() const { return pub_->shared(); }
 
 private:
-  // the executor's page-locked tenant table is read by its previous run's stream-ordered upload: rewritten only after that run
-  void setSlots(Executor &ex, const std::vector<int> &slots, void *stream) {
-    if (ex.tenantsAre(slots.data(), (int)slots.size())) return;
+  // the executor's page-locked tenant and c1 tables are read by its previous run's stream-ordered uploads: rewritten only after that
+  // run (c1 empty: no c1 cache)
+  void setSlots(Executor &ex, const std::vector<int> &slots, const std::vector<int> &c1, void *stream) {
+    if (ex.tenantsAre(slots.data(), (int)slots.size()) && (c1.empty() || ex.c1RowsAre(c1.data(), (int)c1.size()))) return;
     shared()->dev->sync(stream);
     ex.setTenants(slots.data(), (int)slots.size());
+    if (!c1.empty()) ex.setC1Rows(c1.data(), (int)c1.size());
   }
   std::string rotationKeys_, hoistConstants_, keyStorage_;
   std::unique_ptr<B200Public> pub_;

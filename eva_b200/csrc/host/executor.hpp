@@ -39,6 +39,12 @@ struct KeySeededGuard {
   explicit KeySeededGuard(bool on) { check(evab_set_key_seeded(on ? 1 : 0)); }
   ~KeySeededGuard() { evab_set_key_seeded(0); }
 };
+// scoped evab_set_key_c1_rows: batch instance b of the key switches issued by this thread reads cached c1 rows from region
+// d_region[b] of the key bank, or draws them (-1); null: every instance draws
+struct KeyC1Guard {
+  explicit KeyC1Guard(const std::int32_t *d_region) { check(evab_set_key_c1_rows(d_region)); }
+  ~KeyC1Guard() { evab_set_key_c1_rows(nullptr); }
+};
 
 // Evaluation keys of up to `capacity` tenants (one client's key set each) in one device allocation.  Every tenant's region has
 // the same layout -- the relinearization key, one Galois key per element of the rotation set, then the hoist constants cadd of
@@ -51,12 +57,19 @@ struct KeySeededGuard {
 // Seeded keys (seededKeys, inline constants only): every key of a region is a self-contained seeded image -- its c0 rows [k-1][k][N],
 // then its 32-byte seed padded to 64 bytes (evab_seeded_key_bytes) -- and the key switches draw the c1 rows from the seed
 // (evab_set_key_seeded).  The compressed host image of a tenant is the region's own layout, so a fill is one upload and no launch.
+// c1 regions (c1Regions, seeded keys only): the allocation continues with that many regions of the same stride after the capacity
+// slots; region capacity + h holds the expanded c1 rows of one tenant's keys, key i's rows [k-1][k][N] at the word offset of its c0
+// rows in a seeded image (fillC1, evab_expand_seeded_c1), and an instance whose c1 table entry is capacity + h reads them
+// (evab_set_key_c1_rows) instead of drawing them.
 class KeyBank {
 public:
-  KeyBank(std::shared_ptr<Device> dev, const std::set<u64> &elts, int capacity, bool inlineConstants = false, bool seededKeys = false)
-      : dev_(std::move(dev)), elts_(elts.begin(), elts.end()), inline_(inlineConstants), seeded_(seededKeys) {
+  KeyBank(std::shared_ptr<Device> dev, const std::set<u64> &elts, int capacity, bool inlineConstants = false, bool seededKeys = false,
+          int c1Regions = 0)
+      : dev_(std::move(dev)), elts_(elts.begin(), elts.end()), inline_(inlineConstants), seeded_(seededKeys), c1Regions_(c1Regions) {
     if (capacity < 1 || capacity > 65535) throw std::invalid_argument("key bank capacity must be in [1, 65535]");
     if (seeded_ && !inline_) throw std::invalid_argument("a bank of seeded keys forms its hoist constants inline");
+    if (c1Regions_ < 0 || c1Regions_ > capacity || (c1Regions_ && !seeded_))
+      throw std::invalid_argument("c1 regions: 0 .. capacity, and only in a bank of seeded keys");
     const std::size_t N = dev_->N(), k = (std::size_t)dev_->k();
     if (k < 2) throw std::invalid_argument("a key bank needs at least two primes");
     keyWords_ = seeded_ ? evab_seeded_key_bytes(dev_->ctx()) / 8 : (k - 1) * 2 * k * N;
@@ -64,7 +77,7 @@ public:
       for (std::size_t ell = 1; ell < k; ell++) constWords_ += 2 * (ell + 1) * N;
     stride_ = keyWords_ * (1 + elts_.size()) + constWords_ * elts_.size();
     for (u64 e : elts_) check(evab_galois_prepare(dev_->ctx(), e));
-    bank_ = DBuf(dev_, stride_ * (std::size_t)capacity);
+    bank_ = DBuf(dev_, stride_ * ((std::size_t)capacity + (std::size_t)c1Regions_));
     if (!seeded_) seeds_ = DBuf(dev_, 4 * keys() * (std::size_t)capacity);
     if (!elts_.empty() && !inline_) tmp_ = DBuf(dev_, evab_rotate_hoist_const_levels_work_bytes(dev_->ctx(), (int)elts_.size()) / 8);
     if (!elts_.empty() && inline_) {
@@ -76,7 +89,12 @@ public:
   }
   bool inlineConstants() const { return inline_; }
   bool seededKeys() const { return seeded_; }
-  // the indicator rows [k][N] of an element (inline constants; one copy for every tenant)
+  int c1Regions() const { return c1Regions_; }
+  // the c1 rows of every key of the tenant in slot `slot` -> c1 region h (one launch, stream-ordered; the slot's images must be there)
+  void fillC1(int h, int slot, void *stream) {
+    if (h < 0 || h >= c1Regions_) throw std::logic_error("c1 region out of range");
+    check(evab_expand_seeded_c1(dev_->ctx(), (int)keys(), region(slot), region(capacity() + h), stream));
+  }  // the indicator rows [k][N] of an element (inline constants; one copy for every tenant)
   const u64 *indicators(u64 elt) const {
     if (!inline_) throw std::logic_error("indicator rows are kept by banks with inline hoist constants only");
     return ind_.get() + index(elt) * (std::size_t)dev_->k() * dev_->N();
@@ -199,6 +217,7 @@ private:
   std::vector<u64> elts_;                 // sorted
   bool inline_ = false;                   // inline hoist constants: no constants in the regions, ind_ holds the indicator rows
   bool seeded_ = false;                   // seeded keys: keyWords_ is one seeded image, no seeds_ (the seeds are in the images)
+  int c1Regions_ = 0;                     // c1 regions after the capacity slots (seeded keys)
   std::size_t keyWords_ = 0, constWords_ = 0, stride_ = 0;   // one key; the constants of one element; one tenant
   std::vector<char> used_;                // 0: free, 1: keys added in full, 2: added compressed
   std::uint64_t fills_ = 0;               // regions filled (keys uploaded, constants computed)
@@ -217,6 +236,7 @@ public:
     if (graph_) evab_graph_destroy(dev_->ctx(), graph_);
     if (hostFlags_) evab_host_free(hostFlags_);
     if (tenantHost_) evab_host_free(tenantHost_);
+    if (c1Host_) evab_host_free(c1Host_);
     for (void *e : events_) evab_event_destroy(dev_->ctx(), e);
     for (void *s : streams_) evab_stream_destroy(dev_->ctx(), s);
   }
@@ -251,9 +271,17 @@ public:
     for (int b = 0; b < n; b++) tenantHost_[b] = tenants[b];
   }
   bool tenantsAre(const int *tenants, int n) const { return bank_ && n == plan_.opt.batch && std::equal(tenants, tenants + n, tenantHost_); }
+  // the c1 table entry of every instance of the next runs (banks with c1 regions): capacity + h, or -1 (draws).  Rewritten under the
+  // same rule as the tenant table
+  void setC1Rows(const int *regions, int n) {
+    if (!c1Host_ || n != plan_.opt.batch) throw std::logic_error("setC1Rows: one entry per instance of a plan bound to a bank with c1 regions");
+    for (int b = 0; b < n; b++) c1Host_[b] = regions[b];
+  }
+  bool c1RowsAre(const int *regions, int n) const { return c1Host_ && n == plan_.opt.batch && std::equal(regions, regions + n, c1Host_); }
   void run(void *stream) {
     if (rawDirty_) { evalRawAndEncodes(stream); rawDirty_ = false; }
     if (bank_) dev_->upload(tenantDev_.get(), tenantHost_, 4 * (std::size_t)plan_.opt.batch, stream);   // read by the kernels, not baked into the graph
+    if (c1Host_) dev_->upload(c1Dev_.get(), c1Host_, 4 * (std::size_t)plan_.opt.batch, stream);
     if (plan_.opt.useGraph && verbosity() < 2) {   // debug verbosity: step-by-step replay so that every term is reported
       if (!graph_ || !graphValid_) capture();
       check(evab_graph_launch(dev_->ctx(), graph_, stream));
@@ -334,6 +362,11 @@ private:
       tenantDev_ = DBuf(dev_, ((std::size_t)B + 1) / 2);
       check(evab_host_alloc(4 * (std::size_t)B, (void **)&tenantHost_));
       std::fill(tenantHost_, tenantHost_ + B, 0);
+      if (bank_->c1Regions()) {
+        c1Dev_ = DBuf(dev_, ((std::size_t)B + 1) / 2);
+        check(evab_host_alloc(4 * (std::size_t)B, (void **)&c1Host_));
+        std::fill(c1Host_, c1Host_ + B, -1);
+      }
       dev_->sync();
     }
   }
@@ -560,6 +593,7 @@ private:
     KeyBankGuard kg(bank_ ? reinterpret_cast<const std::int32_t *>(tenantDev_.get()) : nullptr, bank_ ? bank_->stride() : 0);
     HoistInlineGuard hg(bank_ && bank_->inlineConstants());
     KeySeededGuard sg(bank_ && bank_->seededKeys());
+    KeyC1Guard cg(c1Host_ ? reinterpret_cast<const std::int32_t *>(c1Dev_.get()) : nullptr);
     void *forkEv = events_[p.numEvents + p.usedStreams];
     for (int b = 0; p.numFlags && b < p.opt.batch; b++)   // zero-coefficient flags of the shared mod-ups
       check(evab_memset_zero(c, arena_.get() + (std::size_t)b * p.stride + p.flagsOff, 8 * p.numFlags * 8, stream));
@@ -597,6 +631,8 @@ private:
   u64 *hostFlags_ = nullptr;                              // page-locked copy of the flags of the last run
   DBuf tenantDev_;                                        // bank-bound: int32 tenant of every instance, read by the kernels
   std::int32_t *tenantHost_ = nullptr;                    // its page-locked source (setTenants)
+  DBuf c1Dev_;                                            // bank with c1 regions: int32 c1 table entry of every instance
+  std::int32_t *c1Host_ = nullptr;                        // its page-locked source (setC1Rows)
   std::unordered_set<std::uint64_t> rawUploaded_;
   bool staticEncoded_ = false;
   DBuf rawArena_;

@@ -194,6 +194,26 @@ PYBIND11_MODULE(_eva_b200, m) {
     }
     return py::make_tuple(results, c.fills(), c.evictions());
   }, py::arg("slots"), py::arg("batches"));
+  // test hook: the c1 cache's admission and eviction policy alone (host/slot_cache.hpp C1Cache), as _slot_cache.  Returns (per entry:
+  // (region of every instance or -1, [(tenant, region, evicted or -1)], the tenants holding a region), or None for a removal;
+  // fills; evictions)
+  m.def("_c1_cache", [](int regions, const std::vector<py::object> &ops) {
+    C1Cache c(regions);
+    py::list results;
+    for (auto &op : ops) {
+      if (py::isinstance<py::tuple>(op)) {   // ("remove", tenant)
+        c.drop(py::cast<int>(op.cast<py::tuple>()[1]));
+        results.append(py::none());
+        continue;
+      }
+      std::vector<C1Cache::Fill> fills;
+      std::vector<int> r = c.assign(op.cast<std::vector<int>>(), fills);
+      py::list fl;
+      for (auto &f : fills) fl.append(py::make_tuple(f.tenant, f.region, f.evicted));
+      results.append(py::make_tuple(r, fl, c.cached()));
+    }
+    return py::make_tuple(results, c.fills(), c.evictions());
+  }, py::arg("regions"), py::arg("batches"));
   // test hook: the planner alone (host/planner.hpp), without a device.  options: set_options' keywords; arena_limit 0 is no limit
   // here.  The scratch sizes are stand-ins derived from N and ell (the layout's invariants hold for any sizes)
   py::class_<ExecOptions> planOptions(m, "_PlanOptions");
@@ -506,10 +526,10 @@ PYBIND11_MODULE(_eva_b200, m) {
                              "Executes compiled programs for many clients: each client's evaluation keys are a tenant of a key bank of fixed "
                              "capacity, the plans are shared by all tenants, and every instance of a batch runs with its own tenant's keys");
   srv.def(py::init([](const CKKSParameters &params, int capacity, int device, std::optional<int> maxTenants, const std::string &rotationKeys,
-                       const std::string &hoistConstants, const std::string &keyStorage) {
-        return std::make_unique<B200Server>(params, capacity, device, maxTenants ? *maxTenants : -1, rotationKeys, hoistConstants, keyStorage);
+                       const std::string &hoistConstants, const std::string &keyStorage, int c1Cache) {
+        return std::make_unique<B200Server>(params, capacity, device, maxTenants ? *maxTenants : -1, rotationKeys, hoistConstants, keyStorage, c1Cache);
       }), py::arg("params"), py::arg("capacity") = 64, py::arg("device") = 0, py::arg("max_tenants") = py::none(), py::arg("rotation_keys") = "program",
-      py::arg("hoist_constants") = "stored", py::arg("key_storage") = "expanded",
+      py::arg("hoist_constants") = "stored", py::arg("key_storage") = "expanded", py::arg("c1_cache") = 0,
       "capacity: device slots (key-bank regions).  max_tenants None or == capacity: a tenant id is its slot, filled when its keys are "
       "added.  max_tenants > capacity: up to max_tenants tenants' keys in page-locked host memory, paged into the slots (least "
       "recently used first) as batches need them.  rotation_keys: the Galois keys every tenant supplies -- \"program\", one per "
@@ -518,7 +538,10 @@ PYBIND11_MODULE(_eva_b200, m) {
       "(computed at every fill); \"inline\", slots hold the keys only and the hoisted rotations form the constants inside the "
       "key-switch inner product (same outputs, smaller slots; approx_hoist is not available).  key_storage: \"expanded\", every key in "
       "full; \"seeded\" (with hoist_constants=\"inline\"), slots hold each key's c0 rows and seed and the key switches draw the uniform "
-      "half from the seed (same outputs, half the slot; compressed keys only)")
+      "half from the seed (same outputs, half the slot; compressed keys only).  c1_cache (key_storage=\"seeded\", 0 <= c1_cache <= "
+      "capacity): device regions, each holding the expanded c1 rows of one tenant; the instances of a batch whose tenant holds one read "
+      "them instead of drawing (same outputs).  The tenants with the most instances in a batch are admitted first, the least recently "
+      "used region is evicted; tenants without a region draw")
       .def("add_raw_keys", [](B200Server &s, const u64arr &relin, const std::map<u64, u64arr> &galois) {
         const std::size_t kk = s.shared()->dev->k(), N = s.shared()->dev->N();
         requireShape(relin, {kk - 1, 2, kk, N}, "relinearization key");
@@ -637,6 +660,12 @@ PYBIND11_MODULE(_eva_b200, m) {
         d["hoist_constants"] = s.hoistConstants();
         d["key_storage"] = s.keyStorage();
         d["indicator_bytes"] = b.indicatorBytes();
+        const C1Store *c1 = s.shared()->c1.get();
+        d["c1_cache"] = b.c1Regions();
+        d["c1_cache_bytes"] = b.stride() * 8 * (std::size_t)b.c1Regions();
+        d["c1_cached"] = c1 ? c1->cache().cached() : std::vector<int>();
+        d["c1_fills"] = c1 ? c1->cache().fills() : 0;
+        d["c1_evictions"] = c1 ? c1->cache().evictions() : 0;
         return d;
       }, "capacity / device_slots: key-bank regions; rotation_keys: the key set of galois_elements (\"program\" or \"power_of_two\"); "
          "hoist_constants: \"stored\" or \"inline\" (then hoist_const_bytes_per_tenant is 0 and indicator_bytes the one shared copy of "
@@ -644,7 +673,8 @@ PYBIND11_MODULE(_eva_b200, m) {
          "max_tenants: tenant ids (more than the slots: paging); resident: the tenants "
          "holding a slot; host_key_bytes: page-locked host memory of the paged keys (compressed tenants: c0 rows and seeds); "
          "compressed_tenants: tenants added in compressed form; fills: slots filled (keys uploaded and "
-         "constants computed); evictions: resident tenants displaced by a fill")
+         "constants computed); evictions: resident tenants displaced by a fill; c1_cache: c1 regions (c1_cache_bytes of device memory); "
+         "c1_cached: the tenants holding one; c1_fills: regions expanded; c1_evictions: cached tenants displaced by a fill")
       .def("primes", [](B200Server &s) { return s.shared()->dev->primes(); })
       // ---- benchmark hooks (as B200Public's): device-resident execution of requests staged on a plan replica
       .def("stage_inputs", [](B200Server &s, Program &prog, const Requests &rq, std::uintptr_t stream, int replica) {

@@ -80,4 +80,80 @@ private:
   std::uint64_t clock_ = 0, fills_ = 0, evictions_ = 0;
 };
 
+// Residency of tenants' cached c1 rows (B200Server c1_cache): which tenant holds which of a seeded bank's c1 regions, and which
+// regions a batch's tenants take.  Unlike bank slots, a batch may name more distinct tenants than there are regions: the tenants
+// left out draw their c1 rows in the kernels, as without a cache.
+class C1Cache {
+public:
+  struct Fill { int tenant, region, evicted; };   // evicted: the tenant the region held before, -1 if it was free
+
+  explicit C1Cache(int regions) : owner_(regions, -1), stamp_(regions, 0) {
+    if (regions < 1) throw std::invalid_argument("a c1 cache needs at least one region");
+  }
+  int regions() const { return (int)owner_.size(); }
+  int regionOf(int tenant) const { auto it = region_.find(tenant); return it == region_.end() ? -1 : it->second; }
+  // tenants holding a region, in region order
+  std::vector<int> cached() const {
+    std::vector<int> r;
+    for (int t : owner_) if (t >= 0) r.push_back(t);
+    return r;
+  }
+  std::uint64_t fills() const { return fills_; }
+  std::uint64_t evictions() const { return evictions_; }
+
+  // The region of every instance of a batch, -1: the instance draws.  Admission order: the tenants with more instances in the batch
+  // first, ties by first appearance; the first regions() of them are admitted.  Admitted tenants that hold a region keep it
+  // (pinned); each missing one, in admission order, takes the lowest free region, else the least recently used region that no
+  // admitted tenant holds.  `fills` receives the regions to fill.  Every instance whose tenant then holds a region reads it -- a
+  // tenant left out of admission keeps its region while no admitted tenant needs it.
+  std::vector<int> assign(const std::vector<int> &tenants, std::vector<Fill> &fills) {
+    std::vector<int> order;           // distinct tenants by first appearance
+    std::unordered_map<int, int> count;
+    for (int t : tenants)
+      if (count[t]++ == 0) order.push_back(t);
+    std::stable_sort(order.begin(), order.end(), [&](int a, int b) { return count[a] > count[b]; });
+    if ((int)order.size() > regions()) order.resize(regions());
+    std::vector<char> pinned(regions(), 0);
+    for (int t : order) if (int r = regionOf(t); r >= 0) pinned[r] = 1;
+    for (int t : order) {
+      if (regionOf(t) >= 0) continue;
+      const int r = victim(pinned);
+      const int old = owner_[r];
+      if (old >= 0) { region_.erase(old); evictions_++; }
+      owner_[r] = t; region_[t] = r; pinned[r] = 1;
+      fills.push_back(Fill{t, r, old});
+      fills_++;
+    }
+    ++clock_;
+    std::vector<int> out;
+    out.reserve(tenants.size());
+    for (int t : tenants) {
+      const int r = regionOf(t);
+      if (r >= 0) stamp_[r] = clock_;
+      out.push_back(r);
+    }
+    return out;
+  }
+  // the tenant's keys are gone: its region (if any) becomes free
+  void drop(int tenant) {
+    auto it = region_.find(tenant);
+    if (it == region_.end()) return;
+    owner_[it->second] = -1; stamp_[it->second] = 0;
+    region_.erase(it);
+  }
+
+private:
+  int victim(const std::vector<char> &pinned) const {
+    for (int r = 0; r < regions(); r++) if (owner_[r] < 0) return r;
+    int best = -1;
+    for (int r = 0; r < regions(); r++)
+      if (!pinned[r] && (best < 0 || stamp_[r] < stamp_[best])) best = r;
+    return best;   // exists: at most regions() tenants are admitted, and one of them is missing
+  }
+  std::vector<int> owner_;                 // region -> tenant, -1: free
+  std::vector<std::uint64_t> stamp_;       // region -> last batch use (LRU)
+  std::unordered_map<int, int> region_;    // tenant -> region
+  std::uint64_t clock_ = 0, fills_ = 0, evictions_ = 0;
+};
+
 }  // namespace evab

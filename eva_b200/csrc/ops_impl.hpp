@@ -207,12 +207,14 @@ int ks_finish(BE &be, const CtxView &c, int ell, u64 *out, const u64 *t, const u
   return divround_impl(be, c, acc, (long long)(ell + 1) * N, 2, ell + 1, pm, sp, out, (long long)ell * N, base, (long long)ell * N, tmp,
                        base_polys, nperm);
 }
+template <class BE> int require_c1_rows(BE &be);
 template <class BE>
 int keyswitch_impl(BE &be, const CtxView &c, int ell, u64 *out, const u64 *t, const u64 *key, const u64 *base, int base_polys, u64 *work,
                    const u64 *that_in = nullptr, const u32 *ctab = nullptr, const u32 *nperm = nullptr) {
   const long long N = (long long)c.N;
   const int k = c.k;
   if (ell < 1 || ell > k - 1) return be.error("key switching needs 1 <= ell <= k-1");
+  if (int rc = require_c1_rows(be)) return rc;
   u64 *that = work;
   u64 *ext = work + ks_off_ext(c, ell);
   u64 *acc = work + ks_off_acc(c, ell);
@@ -322,11 +324,24 @@ template <class BE> bool hoist_inline_of(BE &, long) { return false; }
 // are then formed inline only, and nothing else may read such a key
 template <class BE> auto key_seeded_of(BE &be, int) -> decltype(be.key_seeded()) { return be.key_seeded(); }
 template <class BE> bool key_seeded_of(BE &, long) { return false; }
+// cached c1 rows (evab_set_key_c1_rows): the backend's key_c1_rows() where it has one, else off.  While on, an instance with a c1
+// region reads its keys' c1 rows from it instead of drawing them, which needs seeded keys and a key-bank table (the region offset is
+// a multiple of the bank's stride)
+template <class BE> auto key_c1_rows_of(BE &be, int) -> decltype(be.key_c1_rows()) { return be.key_c1_rows(); }
+template <class BE> bool key_c1_rows_of(BE &, long) { return false; }
+template <class BE> auto key_bank_of(BE &be, int) -> decltype(be.key_bank()) { return be.key_bank(); }
+template <class BE> bool key_bank_of(BE &, long) { return false; }
+template <class BE> int require_c1_rows(BE &be) {
+  if (!key_c1_rows_of(be, 0)) return 0;
+  if (!key_seeded_of(be, 0)) return be.error("cached c1 rows (evab_set_key_c1_rows) need seeded keys: evab_set_key_seeded is off");
+  if (!key_bank_of(be, 0)) return be.error("cached c1 rows (evab_set_key_c1_rows) need a key-bank table: evab_set_key_bank is not set");
+  return 0;
+}
 // the hoisted rotations take inline hoist constants with seeded keys
 template <class BE> int require_seeded_inline(BE &be) {
   if (key_seeded_of(be, 0) && !hoist_inline_of(be, 0))
     return be.error("hoisted rotations with seeded keys (evab_set_key_seeded) need inline hoist constants (evab_set_hoist_inline)");
-  return 0;
+  return require_c1_rows(be);
 }
 inline size_t hoist_const_elems(const CtxView &c, int ell) { return (size_t)2 * (ell + 1) * c.N; }
 // cadd_g for one Galois key at one level; `tmp` holds (ell + 1) * N words
@@ -416,11 +431,17 @@ struct SeedTileHost {
   std::vector<u64> buf;
   int ell = 0, j0 = 0;
   const u64 *cur = nullptr;
+  long long c1off = -1;   // >= 0: the instance's cached c1 rows, at keys[i] + c1off (evab_set_key_c1_rows): copied, not drawn
   void fill(const u64 *const *keys, int n, long long koff, int ell_, int row, int k, size_t N, const PrimeDev &P, int tile_j0) {
     ell = ell_; j0 = tile_j0;
     buf.assign((size_t)n * ell * T, 0);
     const u64 lim = kx_limit(P.p);
     for (int i = 0; i < n; i++) {
+      if (c1off >= 0) {
+        for (int J = 0; J < ell; J++)
+          std::memcpy(buf.data() + ((size_t)i * ell + J) * T, seeded_c0(keys[i] + c1off, J, row, k, N) + j0, (size_t)T * 8);
+        continue;
+      }
       uint32_t seed[8];
       seeded_seed(keys[i] + koff, k, N, seed);
       for (int J = 0; J < ell; J++)
@@ -431,10 +452,11 @@ struct SeedTileHost {
   u64x2 c1(int J, int j) const { return ld2(cur + (size_t)J * T + (j - j0)); }
 };
 // every (row mi, coefficient pair j) of an element body replayed serially; SEED: one tile fill per row and T coefficients, body(mi,
-// j, tile) with the filled tile (nullptr without SEED)
+// j, tile) with the filled tile (nullptr without SEED); c1off >= 0: the instance's cached c1 rows (SeedTileHost::c1off)
 template <bool SEED, class Body>
-void seeded_replay(const u64 *const *keys, int n, long long koff, const PrimeDev *primes, int ell, int k, int N, Body body) {
+void seeded_replay(const u64 *const *keys, int n, long long koff, const PrimeDev *primes, int ell, int k, int N, Body body, long long c1off = -1) {
   SeedTileHost tile;
+  tile.c1off = c1off;
   for (int mi = 0; mi <= ell; mi++) {
     const int row = mi == ell ? k - 1 : mi;
     for (int j0 = 0; j0 < N; j0 += SeedTileHost::T) {
@@ -443,10 +465,13 @@ void seeded_replay(const u64 *const *keys, int n, long long koff, const PrimeDev
     }
   }
 }
-template <int NOUT> void rot_wsum_ip_replay(const WsumIpArgs &A, long long koff, bool inl, bool seeded) {
+// the c1 region offset of a replayed instance: the replay backend's c1_off() where it has one (evab_set_key_c1_rows), else -1 (drawn)
+template <class BE> auto replay_c1_off(BE &be, int) -> decltype(be.c1_off()) { return be.c1_off(); }
+template <class BE> long long replay_c1_off(BE &, long) { return -1; }
+template <int NOUT> void rot_wsum_ip_replay(const WsumIpArgs &A, long long koff, bool inl, bool seeded, long long c1off) {
   if (seeded)
     seeded_replay<true>(A.key, A.n, koff, A.primes, A.ell, A.k, A.N,
-                        [&](int mi, int j, SeedTileHost *t) { rot_wsum_ip_elem<NOUT, true, true>(A, mi, j, 0, koff, t); });
+                        [&](int mi, int j, SeedTileHost *t) { rot_wsum_ip_elem<NOUT, true, true>(A, mi, j, 0, koff, t); }, c1off);
   else
     seeded_replay<false>(A.key, A.n, koff, A.primes, A.ell, A.k, A.N, [&](int mi, int j, SeedTileHost *) {
       if (inl) rot_wsum_ip_elem<NOUT, true>(A, mi, j, 0, koff);
@@ -462,11 +487,12 @@ template <class BE> int rot_wsum_ip_step(BE &be, const WsumIpArgs &A) {
 #else
   const long long koff = replay_key_off(be, 0);
   const bool inl = hoist_inline_of(be, 0), seeded = key_seeded_of(be, 0);   // seeded: inline (require_seeded_inline)
+  const long long c1off = replay_c1_off(be, 0);
   switch (A.nout) {
-    case 1: rot_wsum_ip_replay<1>(A, koff, inl, seeded); break;
-    case 2: rot_wsum_ip_replay<2>(A, koff, inl, seeded); break;
-    case 3: rot_wsum_ip_replay<3>(A, koff, inl, seeded); break;
-    case 4: rot_wsum_ip_replay<4>(A, koff, inl, seeded); break;
+    case 1: rot_wsum_ip_replay<1>(A, koff, inl, seeded, c1off); break;
+    case 2: rot_wsum_ip_replay<2>(A, koff, inl, seeded, c1off); break;
+    case 3: rot_wsum_ip_replay<3>(A, koff, inl, seeded, c1off); break;
+    case 4: rot_wsum_ip_replay<4>(A, koff, inl, seeded, c1off); break;
     default: return be.error("rotate_wsum: 1..4 output sums");
   }
   return 0;
@@ -565,6 +591,7 @@ int lazy_rotsum_impl(BE &be, const CtxView &c, int ell, int nout, u64 *out, cons
                      const u64 *const *keys, const u64 *const *cadds, const u64 *const *wts, u64 *work) {
   if (hoist_inline_of(be, 0)) return be.error("lazy_rotsum (approx_hoist) takes stored hoist constants: turn evab_set_hoist_inline off");
   if (key_seeded_of(be, 0)) return be.error("lazy_rotsum (approx_hoist) reads expanded keys: turn evab_set_key_seeded off");
+  if (int rc = require_c1_rows(be)) return rc;
   if (ell < 1 || ell > c.k - 1) return be.error("lazy_rotsum needs 1 <= ell <= k-1");
   if (n < 1 || n > LRS_MAX) return be.error("lazy_rotsum: 1..16 rotations");
   if (nout < 1 || nout > LRS_OUT) return be.error("lazy_rotsum: 1..4 output sums");

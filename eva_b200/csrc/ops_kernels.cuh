@@ -215,6 +215,15 @@ EVAB_HD void seeded_seed(const u64 *key, int k, size_t N, uint32_t (&seed)[8]) {
 #pragma unroll
   for (int i = 0; i < 8; i++) seed[i] = s[i];
 }
+// evab_expand_seeded_c1: coefficients 8 t .. 8 t + 7 of c1 row r = J k + m of seeded image i (images seeded_key_words apart) into
+// the c1-region geometry -- the row sits where the image's c0 row (J, m) sits, at rows + i seeded_key_words + r N
+EVAB_HD void expand_seeded_c1_elem(const u64 *images, u64 *rows, const PrimeDev *primes, int k, size_t N, int i, int r, u32 t) {
+  const size_t sw = seeded_key_words(k, N);
+  uint32_t seed[8];
+  seeded_seed(images + (size_t)i * sw, k, N, seed);
+  const PrimeDev &P = primes[r % k];
+  seeded_c1_draw8(seed, r / k, r % k, k, P, kx_limit(P.p), t, rows + (size_t)i * sw + (size_t)r * N + 8 * (size_t)t);
+}
 // expanded keys: no tile (never dereferenced)
 struct SeedTileNone {
   EVAB_HD void begin(int, int, const u64 *, int, int, int, int, const PrimeDev &) {}
@@ -234,11 +243,21 @@ template <bool SEED, class Tile> EVAB_HD void key_words(const u64 *key, const Ti
 // the tile of one thread block in shared memory: [ell][2 blockDim.x] words, coefficients j0 .. j0 + 2 blockDim.x - 1 of the block's
 // row, j0 = j - 2 threadIdx.x.  begin(i, j, ...) is called by every thread of the block with the same key and row (the kernels' tile
 // loops are uniform, N a multiple of the tile): a barrier (the previous tile's readers), ell / 4 ChaCha blocks per thread (rounded
-// up), a barrier
+// up), a barrier.
+// Cached c1 rows (evab_set_key_c1_rows): when the block's instance has a c1 region (`cached`, uniform over the block), its rows
+// [k-1][k][N] sit at the image + c1d words, c0's geometry; each thread then copies its own 2 words of every J < ell into the tile
+// -- read once from memory, nothing drawn, and no barrier, since no other thread reads them
 struct SeedTileDev {
   u64 *s;
+  bool cached = false;
+  long long c1d = 0;
   EVAB_HD void begin(int, int j, const u64 *key, int ell, int row, int k, int N, const PrimeDev &P) {
 #if defined(__CUDA_ARCH__)
+    if (cached) {
+      const u64 *rows = key + c1d;
+      for (int J = 0; J < ell; J++) st2(s + (size_t)J * 2 * blockDim.x + 2 * threadIdx.x, ld2(seeded_c0(rows, J, row, k, N) + j));
+      return;
+    }
     const int T = 2 * blockDim.x, per = T / 8;
     const u32 t0 = (u32)(j - 2 * (int)threadIdx.x) / 8;
     uint32_t seed[8];

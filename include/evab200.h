@@ -109,6 +109,17 @@ int evab_set_hoist_inline(int on);
  * evab_rotate_hoist_const and evab_rotate_hoist_const_levels fail while it is on. */
 int evab_set_key_seeded(int on);
 size_t evab_seeded_key_bytes(const evab_ctx *ctx);
+/* Cached c1 rows, thread-local like evab_set_key_bank (null: off).  d_region_of_instance is a device table of one int32 per batch
+ * instance, read by the kernels at run time (a captured graph follows a rewritten table): instance b with region r = table[b] >= 0
+ * reads the c1 rows of every key it switches with from key operand + r * tenant_stride_words, where key i's c1 rows [k-1][k][N]
+ * sit at the word offset of its c0 rows in a seeded image (evab_expand_seeded_c1 writes them); an instance with r < 0 draws them
+ * from the seed.  The outputs are the same either way.  Valid only while evab_set_key_seeded is on and a key-bank table is set:
+ * otherwise the key-switch calls fail, naming the missing setting. */
+int evab_set_key_c1_rows(const int32_t *d_region_of_instance);
+/* the c1 rows of the n consecutive seeded images at d_images (evab_seeded_key_bytes apart) -> d_rows, in the geometry above: image
+ * i's row (J, m) at d_rows + i * evab_seeded_key_bytes / 8 + (J k + m) N words (the 8 seed words of every image are not written).
+ * Both pointers 64-byte aligned; device memory; stream-ordered */
+int evab_expand_seeded_c1(evab_ctx *ctx, int n, const uint64_t *d_images, uint64_t *d_rows, void *stream);
 /* number of kernel launches issued through this context so far */
 uint64_t evab_launch_count(const evab_ctx *ctx);
 
