@@ -649,4 +649,65 @@ private:
   CKKSConfig config_;
 };
 
+// ---- slot packing: k instances of a compiled program whose vec_size v is below N/2, in every ciphertext ----
+// Instance b's slot i sits at packed slot i*k + b, which fills k*v slots.  A rotation by r*k of the packed vector (period v*k) is
+// the rotation by r of every instance: (i*k + b + r*k) mod (v*k) = ((i + r) mod v)*k + b.  Every other op acts slot by slot.  So the
+// packed program is the same program with vec_size v*k, every rotation step r replaced by (r mod v)*k, and every constant of m values
+// replaced by its m*k interleaved values c'[i*k + b] = c[i] (a uniform constant keeps its one value).  Types, scales, levels, rescales,
+// relinearizations, mod-switches and the input and output names stay.  The parameters keep prime_bits and N, with the packed
+// program's rotation steps; the signature keeps its inputs' encodings with vec_size v*k.  What runs it (planner, executor, keys)
+// sees an ordinary program with the same terms.  k = 1 returns copies of the input.
+inline std::tuple<std::unique_ptr<Program>, CKKSParameters, CKKSSignature> packProgram(const Program &prog, const CKKSParameters &params,
+                                                                                       const CKKSSignature &sig, int k) {
+  const std::size_t v = prog.getVecSize(), slots = params.polyModulusDegree / 2;
+  if (k < 1 || (k & (k - 1))) throw std::invalid_argument("pack_program: k = " + std::to_string(k) + " is not a power of two");
+  if ((std::size_t)sig.vecSize != v)
+    throw std::invalid_argument("pack_program: the signature's vec_size " + std::to_string(sig.vecSize) + " differs from the program's vec_size " + std::to_string(v));
+  if ((std::size_t)k * v > slots)
+    throw std::invalid_argument("pack_program: k = " + std::to_string(k) + " instances of vec_size " + std::to_string(v) + " need " + std::to_string(k * v) +
+                                " slots, more than the " + std::to_string(slots) + " of N = " + std::to_string(params.polyModulusDegree));
+  if (k == 1) return std::make_tuple(prog.deepCopy(), params, sig);
+  auto packed = std::make_unique<Program>(prog.getName() + ".pack" + std::to_string(k), v * k);
+  std::map<const Term *, std::string> inName, outName;
+  for (auto &e : prog.getInputs()) inName[e.second.get()] = e.first;
+  for (auto &e : prog.getOutputs()) outName[e.second.get()] = e.first;
+  std::map<std::uint64_t, Term::Ptr> copy;
+  std::map<std::uint64_t, Type> type;   // the compiler's type deduction: rotation keys are selected for non-Raw rotations only
+  std::set<int> rotations;
+  for (auto &t : prog.toposort()) {
+    std::vector<Term::Ptr> ops;
+    Type ty = Type::Raw;
+    for (auto &o : t->getOperands()) {
+      ops.push_back(copy.at(o->index));
+      if (type.at(o->index) == Type::Cipher) ty = Type::Cipher;
+    }
+    if (t->op == Op::Encode) ty = Type::Plain;
+    else if (t->op == Op::Input) ty = t->type.value();
+    type[t->index] = ty;
+    Term::Ptr n = t->op == Op::Input ? packed->makeInput(inName.at(t.get()), ty)
+                : t->op == Op::Output ? packed->makeOutput(outName.at(t.get()), ops.at(0))
+                : packed->makeTerm(t->op, ops);
+    n->copyAttributesFrom(*t);
+    if (t->op == Op::RotateLeftConst || t->op == Op::RotateRightConst) {
+      const long long r = ((long long)*t->rotation % (long long)v + (long long)v) % (long long)v;
+      n->rotation = (std::int32_t)(r * k);
+      if (ty != Type::Raw) rotations.insert(t->op == Op::RotateLeftConst ? *n->rotation : -*n->rotation);
+    }
+    if (t->constant) {
+      const std::vector<double> &c = t->constant->values();
+      std::vector<double> interleaved;
+      if (c.size() == 1) interleaved = c;
+      else {
+        interleaved.reserve(c.size() * k);
+        for (double x : c) interleaved.insert(interleaved.end(), (std::size_t)k, x);
+      }
+      n->constant = std::make_shared<ConstantValue>(t->constant->size() * k, std::move(interleaved));
+    }
+    copy[t->index] = n;
+  }
+  CKKSParameters pp = params;
+  pp.rotations = rotations;
+  return std::make_tuple(std::move(packed), std::move(pp), CKKSSignature((int)(v * k), sig.inputs));
+}
+
 }  // namespace evab

@@ -266,6 +266,9 @@ PYBIND11_MODULE(_eva_b200, m) {
       .def(py::init<std::unordered_map<std::string, std::string>>(), py::arg("config"), "Create a compiler with a custom config (dict from strings to strings)")
       .def("compile", &CKKSCompiler::compile, py::arg("program"),
            "Compile a program for CKKS; returns (compiled Program, CKKSParameters, CKKSSignature)");
+  mckks.def("pack_program", &packProgram, py::arg("program"), py::arg("params"), py::arg("signature"), py::arg("k"),
+            "k instances of a compiled program in every ciphertext: returns (packed Program, CKKSParameters, CKKSSignature) with "
+            "vec_size k * vec_size; instance b's slot i is packed slot i * k + b (the inputs are left untouched)");
   py::class_<CKKSParameters>(mckks, "CKKSParameters", "Abstract encryption parameters for CKKS")
       .def(py::init([](std::vector<std::uint32_t> bits, std::set<int> rots, std::uint32_t n) { CKKSParameters p; p.primeBits = bits; p.rotations = rots; p.polyModulusDegree = n; return p; }),
            py::arg("prime_bits"), py::arg("rotations"), py::arg("poly_modulus_degree"))
