@@ -52,6 +52,7 @@ _SIGS = {
     "evab_hoist_indicators": (ci, [vp, ci, u64p, vp, vp]),
     "evab_expand_key_uniform": (ci, [vp, ci, vp, u64p, vp, vp]),
     "evab_expand_cipher_uniform": (ci, [vp, ci, vp, vp, vp, u64p, vp]),
+    "evab_gather_ciphers": (ci, [vp, ci, vp, vp, u64p, vp]),
     "evab_rotate_modup_prepared": (ci, [vp, ci, vp, vp, vp, u64, vp, vp, vp, vp]),
     "evab_memset_zero": (ci, [vp, vp, szt, vp]),
     "evab_rotate_modup_scale_c0": (ci, [vp, ci, vp, vp, vp]),

@@ -318,6 +318,29 @@ __global__ void __launch_bounds__(256) k_expand_cipher_uniform(const CipherExpan
   const u32 t = blockIdx.x * blockDim.x + threadIdx.x;
   if (t < A.N / 8 && blockIdx.y < A.e[blockIdx.z].ell) expand_cipher_elem(A, blockIdx.z, blockIdx.y, t);
 }
+// ---- server-resident ciphertexts (evab_gather_ciphers): n device ranges copied into arena slots.  The ranges travel by value in
+// the launch arguments, GW_MAX_ENTRIES per launch under the 4 KB parameter limit, so the call needs no device table and a captured
+// graph replays it as it is
+#define GW_MAX_ENTRIES 160
+#define GW_THREADS 128
+#define GW_UNROLL 4                       // 16-byte vectors in flight per thread
+struct GatherEntry { const u64x2 *src; u64x2 *dst; u64 vecs; };   // vecs: 16-byte vectors (2 words each)
+struct GatherArgs { GatherEntry e[GW_MAX_ENTRIES]; };
+static_assert(sizeof(GatherArgs) <= 4096, "the gather's arguments must fit the classic 4 KB parameter space");
+// grid (tiles of GW_THREADS * GW_UNROLL vectors, entry i of the launch): GW_UNROLL loads in flight, then their stores
+__global__ void __launch_bounds__(GW_THREADS) k_gather_words(const GatherArgs A) {
+  const GatherEntry E = A.e[blockIdx.y];
+  const u64 step = (u64)gridDim.x * GW_THREADS * GW_UNROLL;
+  for (u64 i = (u64)blockIdx.x * GW_THREADS * GW_UNROLL + threadIdx.x; i < E.vecs; i += step) {
+    u64x2 v[GW_UNROLL];
+#pragma unroll
+    for (int u = 0; u < GW_UNROLL; u++)
+      if (i + u * GW_THREADS < E.vecs) v[u] = E.src[i + u * GW_THREADS];
+#pragma unroll
+    for (int u = 0; u < GW_UNROLL; u++)
+      if (i + u * GW_THREADS < E.vecs) E.dst[i + u * GW_THREADS] = v[u];
+  }
+}
 __global__ void __launch_bounds__(256) k_hoist_indicator(u64 *out, const u32 *ctab, int N) {
   for (int j = blockIdx.x * blockDim.x + threadIdx.x; j < N; j += gridDim.x * blockDim.x) hoist_indicator_elem(out, ctab, N, blockIdx.y, j);
 }
@@ -1147,6 +1170,36 @@ extern "C" int evab_expand_cipher_uniform(evab_ctx *c, int n, const uint8_t *see
     }
     c->launches.fetch_add(1, std::memory_order_relaxed);
     k_expand_cipher_uniform<<<dim3((A.N / 8 + 255) / 256, rows, nb), 256, 0, S(stream)>>>(A);
+    CUDA_OK(cudaGetLastError());
+  }
+  return 0;
+}
+extern "C" int evab_gather_ciphers(evab_ctx *c, int n, const uint64_t *const *src, uint64_t *const *dst, const uint64_t *words, void *stream) {
+  if (n < 0) return fail("evab_gather_ciphers: n must be >= 0");
+  if (!src) return fail("evab_gather_ciphers: h_src is null");
+  if (!dst) return fail("evab_gather_ciphers: h_dst is null");
+  if (!words) return fail("evab_gather_ciphers: h_words is null");
+  for (int i = 0; i < n; i++) {
+    const std::string at = "[" + std::to_string(i) + "]";
+    if (!src[i] || reinterpret_cast<uintptr_t>(src[i]) % 16) return fail("evab_gather_ciphers: h_src" + at + " is null or not 16-byte aligned");
+    if (!dst[i] || reinterpret_cast<uintptr_t>(dst[i]) % 16) return fail("evab_gather_ciphers: h_dst" + at + " is null or not 16-byte aligned");
+    if (words[i] % 2) return fail("evab_gather_ciphers: h_words" + at + " must be even (16-byte vectors)");
+  }
+  CUDA_OK(cudaSetDevice(c->device));
+  // in order on the caller's stream, GW_MAX_ENTRIES entries per launch
+  for (int i0 = 0; i0 < n; i0 += GW_MAX_ENTRIES) {
+    const int nb = std::min(GW_MAX_ENTRIES, n - i0);
+    GatherArgs A{};
+    u64 vecs = 0;
+    for (int b = 0; b < nb; b++) {
+      A.e[b].src = reinterpret_cast<const u64x2 *>(src[i0 + b]);
+      A.e[b].dst = reinterpret_cast<u64x2 *>(dst[i0 + b]);
+      A.e[b].vecs = words[i0 + b] / 2;
+      vecs = std::max(vecs, A.e[b].vecs);
+    }
+    const u64 tiles = std::max<u64>(1, std::min<u64>((vecs + GW_THREADS * GW_UNROLL - 1) / (GW_THREADS * GW_UNROLL), 65535));
+    c->launches.fetch_add(1, std::memory_order_relaxed);
+    k_gather_words<<<dim3((unsigned)tiles, nb), GW_THREADS, 0, S(stream)>>>(A);
     CUDA_OK(cudaGetLastError());
   }
   return 0;

@@ -57,7 +57,9 @@ struct HostPlain { HostBuf data; int ell = 0; double scale = 0; };
 // a seed-compressed fresh ciphertext (B200Secret::encrypt): c0 [ell][N] and the seed of c1 (key_expand.cuh, ciphertext rows);
 // always size 2.  A type of its own, so that no reader of HostCipher can take its ell N words for 2 ell N
 struct HostSeededCipher { HostBuf c0; int ell = 0; double scale = 0; KeySeed seed{}; };
-using SchemeValue = std::variant<HostCipher, HostPlain, std::shared_ptr<ConstantValue>, HostSeededCipher>;
+// a reference to a ciphertext held in a B200Server's store (CipherStore): the handle alone; level, scale and words are the entry's
+struct StoredCipher { std::uint64_t handle = 0; };
+using SchemeValue = std::variant<HostCipher, HostPlain, std::shared_ptr<ConstantValue>, HostSeededCipher, StoredCipher>;
 
 class B200Valuation {
 public:
@@ -242,6 +244,117 @@ private:
   void *stream_ = nullptr;                          // fills
 };
 
+// Server-resident input ciphertexts (B200Server store_entries): one device allocation of `capacity` entries of 2 (k-1) N words,
+// each holding one tenant's size-2 ciphertext [2][ell][N] at its level.  A request names an entry by handle where it would carry
+// the ciphertext, and staging copies the entry into the arena (evab_gather_ciphers).  Handles increase and are never reused, so a
+// released handle, or one of a tenant whose keys were removed (its entries go with them), names nothing afterwards.  Entries do
+// not depend on key residency.  A fill runs on the store's own stream and is synchronised before store() returns; it first waits
+// for the gathers that may still read a released entry (one event per staging stream, recorded after its last gather).
+class CipherStore {
+public:
+  struct Entry { int tenant = -1, ell = 0; double scale = 0; std::uint64_t handle = 0; };   // handle 0: free
+  CipherStore(std::shared_ptr<Device> dev, int capacity)
+      : dev_(std::move(dev)), entries_(capacity), words_(dev_, (std::size_t)capacity * entryWords()) {
+    check(evab_stream_create(dev_->ctx(), &stream_));
+  }
+  ~CipherStore() {
+    evab_ctx *c = dev_->ctx();
+    evab_sync(c, stream_);
+    for (auto &e : gatherEv_) evab_event_destroy(c, e.second);
+    evab_stream_destroy(c, stream_);
+  }
+  CipherStore(const CipherStore &) = delete;
+  int capacity() const { return (int)entries_.size(); }
+  int used() const { return (int)slotOf_.size(); }
+  std::size_t entryWords() const { return 2 * (std::size_t)(dev_->k() - 1) * dev_->N(); }
+  // every value of `v` into a free entry of `tenant`, all or nothing: full size-2 ciphertexts are uploaded, seeded ones have their
+  // c0 uploaded and their c1 drawn into the entry once.  Returns name -> handle
+  std::map<std::string, std::uint64_t> store(int tenant, const B200Valuation &v) {
+    const u64 N = dev_->N();
+    const int k = dev_->k();
+    for (auto &kv : v) {
+      const std::string what = "value " + kv.first;
+      if (auto *c = std::get_if<HostCipher>(&kv.second)) {
+        if (c->size != 2 || c->ell < 1 || c->ell > k - 1 || c->data.size() != (std::size_t)2 * c->ell * N)
+          throw std::invalid_argument(what + ": only size-2 ciphertexts of the server's parameters can be stored");
+      } else if (auto *sc = std::get_if<HostSeededCipher>(&kv.second)) {
+        if (sc->ell < 1 || sc->ell > k - 1 || sc->c0.size() != (std::size_t)sc->ell * N)
+          throw std::invalid_argument(what + ": seeded ciphertext does not match the server's parameters (level / degree)");
+      } else {
+        const char *kind = std::holds_alternative<HostPlain>(kv.second) ? "a plaintext" : std::holds_alternative<StoredCipher>(kv.second) ? "a stored reference" : "a raw vector";
+        throw std::invalid_argument(what + " is " + kind + ": only ciphertexts can be stored");
+      }
+    }
+    if (capacity() - used() < (int)v.size())
+      throw std::invalid_argument("the ciphertext store has " + std::to_string(capacity() - used()) + " free entries of store_entries=" +
+                                  std::to_string(capacity()) + " and the valuation holds " + std::to_string(v.size()) + ": release entries first");
+    evab_ctx *c = dev_->ctx();
+    for (auto &e : gatherEv_) check(evab_stream_wait_event(c, stream_, e.second));
+    std::vector<int> slots;
+    for (int i = 0; i < capacity() && slots.size() < v.size(); i++) if (!entries_[i].handle) slots.push_back(i);
+    std::vector<KeySeed> seeds;
+    std::vector<u64 *> c1;
+    std::vector<int> ells;
+    std::size_t i = 0;
+    for (auto &kv : v) {
+      u64 *dst = words_.get() + slots[i++] * entryWords();
+      if (auto *hc = std::get_if<HostCipher>(&kv.second)) {
+        dev_->upload(dst, hc->data.data(), hc->data.size() * 8, stream_);
+      } else {
+        auto &sc = std::get<HostSeededCipher>(kv.second);
+        dev_->upload(dst, sc.c0.data(), sc.c0.size() * 8, stream_);
+        seeds.push_back(sc.seed); c1.push_back(dst + sc.c0.size()); ells.push_back(sc.ell);
+      }
+    }
+    if (!seeds.empty()) expandCiphers(*dev_, (int)seeds.size(), seeds.data(), c1.data(), ells.data(), stream_);
+    check(evab_sync(c, stream_));   // the first request that names an entry needs no event
+    std::map<std::string, std::uint64_t> out;
+    i = 0;
+    for (auto &kv : v) {
+      const int slot = slots[i++];
+      Entry &e = entries_[slot];
+      e.tenant = tenant; e.handle = next_++;
+      if (auto *hc = std::get_if<HostCipher>(&kv.second)) { e.ell = hc->ell; e.scale = hc->scale; }
+      else { auto &sc = std::get<HostSeededCipher>(kv.second); e.ell = sc.ell; e.scale = sc.scale; }
+      slotOf_[e.handle] = slot;
+      out[kv.first] = e.handle;
+    }
+    return out;
+  }
+  // null: no such entry (never issued, or released)
+  const Entry *find(std::uint64_t handle) const {
+    auto it = slotOf_.find(handle);
+    return it == slotOf_.end() ? nullptr : &entries_[it->second];
+  }
+  const u64 *words(std::uint64_t handle) const { return words_.get() + (std::size_t)slotOf_.at(handle) * entryWords(); }
+  void release(std::uint64_t handle) {
+    auto it = slotOf_.find(handle);
+    if (it == slotOf_.end()) throw std::invalid_argument("handle " + std::to_string(handle) + " names no stored ciphertext (never issued, or released)");
+    entries_[it->second] = Entry();
+    slotOf_.erase(it);
+  }
+  void dropTenant(int tenant) {
+    for (auto it = slotOf_.begin(); it != slotOf_.end();)
+      if (entries_[it->second].tenant == tenant) { entries_[it->second] = Entry(); it = slotOf_.erase(it); }
+      else ++it;
+  }
+  // `stream` has enqueued gathers from the store: a later fill waits for them
+  void afterGather(void *stream) {
+    void *&ev = gatherEv_[stream];
+    if (!ev) check(evab_event_create(dev_->ctx(), &ev));
+    check(evab_event_record(dev_->ctx(), ev, stream));
+  }
+
+private:
+  std::shared_ptr<Device> dev_;
+  std::vector<Entry> entries_;
+  DBuf words_;                                      // [capacity][2 (k-1) N]
+  std::map<std::uint64_t, int> slotOf_;             // live handle -> entry
+  std::map<void *, void *> gatherEv_;               // staging stream -> event after its last gather
+  void *stream_ = nullptr;                          // fills
+  std::uint64_t next_ = 1;
+};
+
 struct Shared {
   std::shared_ptr<Device> dev;
   std::unique_ptr<CkksClient> client;
@@ -249,6 +362,7 @@ struct Shared {
   std::unique_ptr<KeyBank> bank;   // B200Server: the tenants' keys (then `keys` is empty and every batch names a tenant per instance)
   std::unique_ptr<KeyPager> pager; // B200Server with max_tenants > capacity: tenants paged into the bank's regions
   std::unique_ptr<C1Store> c1;     // B200Server with c1_cache > 0: cached c1 rows of a seeded bank (declared after pager: destroyed first)
+  std::unique_ptr<CipherStore> store;   // B200Server with store_entries > 0: the tenants' stored input ciphertexts
   std::mutex execMutex;   // serialises execute / executeMany callers of one context (see executeMany), and key-bank changes
   void requireTenant(int t) const { if (pager) pager->requireRegistered(t); else bank->requireOccupied(t); }
   // the bank region of every instance (with paging: resolved, and missing tenants' fills enqueued)
@@ -360,12 +474,16 @@ public:
   // upload the host inputs of a chunk's nb valuations into the executor's arena (instance b from inputs[b]; H2D on `stream`).
   // Client-supplied valuations are untrusted (they may come from a file): every buffer is checked against the shape the plan
   // expects before its copy.  A seeded ciphertext's c0 is uploaded like any other input; the c1 rows of all of the chunk's seeded
-  // ciphertexts are then expanded on the device by one evab_expand_cipher_uniform call.
+  // ciphertexts are then expanded on the device by one evab_expand_cipher_uniform call.  The chunk's stored inputs (references
+  // checked by checkStored before the batch was enqueued) are copied from the store by one evab_gather_ciphers call.
   void stageInputs(Executor &ex, Program &program, const B200Valuation *const *inputs, int nb, void *stream) {
     const u64 N = s_->dev->N();
     std::vector<KeySeed> seeds;
     std::vector<u64 *> c1;
     std::vector<int> ells;
+    std::vector<const u64 *> gatherSrc;
+    std::vector<u64 *> gatherDst;
+    std::vector<u64> gatherWords;
     for (int b = 0; b < nb; b++)
       for (auto &in : *inputs[b]) {
         auto term = program.getInput(in.first);
@@ -380,6 +498,9 @@ public:
           u64 *dst = ex.valuePtr(term, b);
           s_->dev->upload(dst, sc->c0.data(), sc->c0.size() * 8, stream);
           seeds.push_back(sc->seed); c1.push_back(dst + sc->c0.size()); ells.push_back(sc->ell);
+        } else if (auto *r = std::get_if<StoredCipher>(&in.second)) {
+          if (!s_->store || !s_->store->find(r->handle)) throw std::logic_error("input " + in.first + ": stored reference staged without checkStored");
+          gatherSrc.push_back(s_->store->words(r->handle)); gatherDst.push_back(ex.valuePtr(term, b)); gatherWords.push_back((u64)2 * vi.ell * N);
         } else if (auto *p = std::get_if<HostPlain>(&in.second)) {
           if (vi.kind != Kind::Plain || p->ell != vi.ell || p->data.size() != (std::size_t)vi.ell * N)
             throw std::runtime_error("input " + in.first + ": plaintext does not match the program signature");
@@ -394,8 +515,42 @@ public:
       }
     // One launch for the chunk, on the chunk's stream, before its run.  Stream order gives the rest: the expansion starts after the
     // replica's previous run has stopped reading the arena, a collect() redo (the zero-digit case) stages again and so expands the
-    // same words again, and a packed arena never lends an input's storage to another value (inputs are pinned).
+    // same words again, and a packed arena never lends an input's storage to another value (inputs are pinned).  The same holds
+    // for the gather of stored inputs, whose entries cannot be released while a batch that names them is uncollected.
     if (!seeds.empty()) expandCiphers(*s_->dev, (int)seeds.size(), seeds.data(), c1.data(), ells.data(), stream);
+    if (!gatherSrc.empty()) {
+      check(evab_gather_ciphers(s_->dev->ctx(), (int)gatherSrc.size(), gatherSrc.data(), gatherDst.data(), gatherWords.data(), stream));
+      s_->store->afterGather(stream);
+    }
+  }
+  // Stored inputs come from outside the program as much as inline ones.  Before anything of a batch is enqueued, every reference
+  // is checked: the handle names an entry, the entry belongs to the tenant of the instance that names it (tenants[b]; null without
+  // a key bank), and its level and size are the input's in the plan, as stageInputs checks an inline ciphertext
+  void checkStored(const Executor &ex, Program &program, const B200Valuation *const *inputs, const int *tenants, int nb) const {
+    for (int b = 0; b < nb; b++)
+      for (auto &in : *inputs[b]) {
+        auto *r = std::get_if<StoredCipher>(&in.second);
+        if (!r) continue;
+        const std::string what = "input " + in.first + " (stored ciphertext, handle " + std::to_string(r->handle) + ")";
+        if (!s_->store || !tenants) throw std::invalid_argument(what + ": this context has no ciphertext store (a B200Server with store_entries > 0 has one)");
+        const std::string who = " of tenant " + std::to_string(tenants[b]);
+        const CipherStore::Entry *e = s_->store->find(r->handle);
+        if (!e) throw std::invalid_argument(what + who + ": no such entry (never issued, released, or its tenant's keys were removed)");
+        if (e->tenant != tenants[b]) throw std::invalid_argument(what + who + ": the entry belongs to another tenant");
+        const ValueInfo &vi = ex.info(program.getInput(in.first));
+        if (vi.kind != Kind::Cipher || vi.size != 2 || vi.ell != e->ell)
+          throw std::invalid_argument(what + who + ": the stored ciphertext (size 2, ell " + std::to_string(e->ell) + ") does not match the program signature (" +
+                                      (vi.kind == Kind::Cipher ? "size " + std::to_string(vi.size) + ", ell " + std::to_string(vi.ell) : std::string("not a ciphertext")) + ")");
+      }
+  }
+  // with execMutex held: does a submitted, not yet collected batch name this stored ciphertext?
+  bool storedInFlightLocked(std::uint64_t handle) const {
+    for (auto &w : inFlight_)
+      if (auto p = w.lock(); p && !p->collected)
+        for (const B200Valuation *v : p->inputs)
+          for (auto &in : *v)
+            if (auto *r = std::get_if<StoredCipher>(&in.second); r && r->handle == handle) return true;
+    return false;
   }
   // plans and arenas are cached on the Program: a call that omits an input would silently compute on the previous
   // call's ciphertext.  The reference builds a fresh executor per call and fails on the missing value
@@ -493,6 +648,7 @@ public:
         R = (int)std::max<std::size_t>(1, std::min<std::size_t>((std::size_t)R, have + extra));
       }
       if (const char *cap = std::getenv("EVAB_MAX_REPLICAS")) R = std::max(1, std::min(R, std::atoi(cap)));   // tests / tuning
+      checkStored(first, program, inputs.data(), p.tenants.empty() ? nullptr : p.tenants.data(), B);
     }
     std::vector<char> busy(R, 0);
     // key-bank region of every instance, resolved at every enqueue (so that collect's redo refills a tenant evicted meanwhile)
@@ -572,9 +728,11 @@ public:
   // inside the key-switch inner products (KeyBank).  keyStorage: "expanded" -- every key in full; "seeded" (inline constants only) --
   // c0 rows and seeds, the key switches draw the c1 rows (KeyBank).  c1Cache (seeded keys, 0 .. capacity): regions holding the
   // expanded c1 rows of the tenants used most (C1Store); 0 is the plain seeded bank
+  // storeEntries: entries of the ciphertext store (CipherStore), 0 for none
   B200Server(const CKKSParameters &params, int capacity, int device, int maxTenants = -1, const std::string &rotationKeys = "program",
-             const std::string &hoistConstants = "stored", const std::string &keyStorage = "expanded", int c1Cache = 0)
+             const std::string &hoistConstants = "stored", const std::string &keyStorage = "expanded", int c1Cache = 0, int storeEntries = 0)
       : rotationKeys_(rotationKeys), hoistConstants_(hoistConstants), keyStorage_(keyStorage) {
+    if (storeEntries < 0) throw std::invalid_argument("store_entries (" + std::to_string(storeEntries) + ") must be >= 0");
     if (hoistConstants != "stored" && hoistConstants != "inline")
       throw std::invalid_argument("hoist_constants must be \"stored\" or \"inline\", not \"" + hoistConstants + "\"");
     if (keyStorage != "expanded" && !(keyStorage == "seeded" && hoistConstants == "inline"))
@@ -601,8 +759,24 @@ public:
     s->bank = std::make_unique<KeyBank>(s->dev, elts, capacity, hoistConstants == "inline", keyStorage == "seeded", c1Cache);
     if (maxTenants > capacity) s->pager = std::make_unique<KeyPager>(s->dev, *s->bank, maxTenants);
     if (c1Cache > 0) s->c1 = std::make_unique<C1Store>(s->dev, *s->bank, s->pager.get());
+    if (storeEntries > 0) s->store = std::make_unique<CipherStore>(s->dev, storeEntries);
     pub_ = std::make_unique<B200Public>(s);
   }
+  // the ciphertexts of `enc` (full or seeded) into the store as `tenant`'s entries, all or nothing: name -> handle
+  std::map<std::string, std::uint64_t> store(int tenant, const B200Valuation &enc) {
+    std::lock_guard<std::mutex> guard(shared()->execMutex);
+    requireStore();
+    shared()->requireTenant(tenant);
+    return shared()->store->store(tenant, enc);
+  }
+  void release(std::uint64_t handle) {
+    std::lock_guard<std::mutex> guard(shared()->execMutex);
+    requireStore();
+    if (pub_->storedInFlightLocked(handle))   // collect's redo stages the batch's inputs again
+      throw std::runtime_error("stored ciphertext " + std::to_string(handle) + " is used by a batch that has not been collected");
+    shared()->store->release(handle);
+  }
+  const CipherStore *cipherStore() const { return shared()->store.get(); }
   // host images [k-1][2][k][N] (shapes checked by the caller); every element of the rotation set must be present
   int addKeys(const u64 *relin, const std::map<u64, const u64 *> &galois) {
     if (bank().seededKeys())
@@ -628,6 +802,7 @@ public:
     shared()->requireTenant(t);
     if (pub_->tenantInFlightLocked(t)) throw std::runtime_error("tenant " + std::to_string(t) + " is used by a batch that has not been collected");
     if (shared()->c1) shared()->c1->drop(t);   // an id reused with new keys never reads this tenant's rows
+    if (shared()->store) shared()->store->dropTenant(t);   // nor its stored ciphertexts
     if (shared()->pager) shared()->pager->remove(t);
     else shared()->bank->remove(t);
   }
@@ -639,11 +814,12 @@ public:
     std::lock_guard<std::mutex> guard(shared()->execMutex);
     for (int t : tenants) shared()->requireTenant(t);
     Executor &ex = pub_->executorFor(prog, (int)rq.size(), replica);
+    std::vector<const B200Valuation *> in;
+    for (auto &r : rq) in.push_back(r.second);
+    pub_->checkStored(ex, prog, in.data(), tenants.data(), (int)in.size());
     staged_[&ex] = tenants;
     const std::vector<int> slots = shared()->slotsFor(tenants);
     setSlots(ex, slots, shared()->c1For(tenants, slots), stream);
-    std::vector<const B200Valuation *> in;
-    for (auto &r : rq) in.push_back(r.second);
     pub_->stageInputs(ex, prog, in.data(), (int)in.size(), stream);
   }
   // tenants: replaces the staged tenants of the replica (same count)
@@ -689,6 +865,9 @@ public:
 private:
   // the executor's page-locked tenant and c1 tables are read by its previous run's stream-ordered uploads: rewritten only after that
   // run (c1 empty: no c1 cache)
+  void requireStore() const {
+    if (!shared()->store) throw std::invalid_argument("this server has no ciphertext store: build it with store_entries > 0");
+  }
   void setSlots(Executor &ex, const std::vector<int> &slots, const std::vector<int> &c1, void *stream) {
     if (ex.tenantsAre(slots.data(), (int)slots.size()) && (c1.empty() || ex.c1RowsAre(c1.data(), (int)c1.size()))) return;
     shared()->dev->sync(stream);
@@ -739,6 +918,9 @@ public:
         DBuf pt(s_->dev, (std::size_t)p->ell * N);
         s_->dev->upload(pt.get(), p->data.data(), (std::size_t)p->ell * N * 8);
         out[e.first] = encoder.decode(pt.get(), p->ell, p->scale);
+      } else if (auto *r = std::get_if<StoredCipher>(&e.second)) {
+        throw std::invalid_argument("value " + e.first + " is a reference to a stored ciphertext (handle " + std::to_string(r->handle) +
+                                    "): only a server's requests can name one");
       } else {
         std::get<std::shared_ptr<ConstantValue>>(e.second)->expandTo(out[e.first], sig.vecSize);
       }

@@ -330,8 +330,13 @@ PYBIND11_MODULE(_eva_b200, m) {
           std::memcpy(a.mutable_data(), sc->c0.data(), sc->c0.size() * 8);
           return py::make_tuple("seeded_cipher", a, sc->scale);
         }
+        if (auto *r = std::get_if<StoredCipher>(&sv)) return py::make_tuple("stored", r->handle, py::none());
         return py::make_tuple("raw", std::get<std::shared_ptr<ConstantValue>>(sv)->values(), 0.0);
-      });
+      })
+      .def("set_stored", [](B200Valuation &v, const std::string &name, std::uint64_t handle) { v[name] = StoredCipher{handle}; },
+           py::arg("name"), py::arg("handle"),
+           "a reference to a ciphertext in a B200Server's store (B200Server.store returns the handles): the server stages the stored "
+           "entry where this valuation would carry the ciphertext");
 
   py::class_<PyPending, std::shared_ptr<PyPending>>(mb, "PendingBatch", "a submitted, not yet collected execute_batch");
   py::class_<B200Public> pub(mb, "B200Public", "The public part of the context: encryption and execution on the GPU");
@@ -395,6 +400,7 @@ PYBIND11_MODULE(_eva_b200, m) {
       // ---- benchmark hooks: device-resident execution on a caller-provided stream
       .def("stage_inputs", [](B200Public &p, Program &prog, const std::vector<const B200Valuation *> &in, std::uintptr_t stream, int replica) {
         Executor &ex = p.executorFor(prog, (int)in.size(), replica);
+        p.checkStored(ex, prog, in.data(), nullptr, (int)in.size());   // rejects stored references: a context has no store
         p.stageInputs(ex, prog, in.data(), (int)in.size(), (void *)stream);
       }, py::arg("program"), py::arg("inputs"), py::arg("stream"), py::arg("replica") = 0)
       .def("run_resident", [](B200Public &p, Program &prog, std::uintptr_t stream, int batch, int replica) { p.executorFor(prog, batch, replica).run((void *)stream); },
@@ -529,10 +535,11 @@ PYBIND11_MODULE(_eva_b200, m) {
                              "Executes compiled programs for many clients: each client's evaluation keys are a tenant of a key bank of fixed "
                              "capacity, the plans are shared by all tenants, and every instance of a batch runs with its own tenant's keys");
   srv.def(py::init([](const CKKSParameters &params, int capacity, int device, std::optional<int> maxTenants, const std::string &rotationKeys,
-                       const std::string &hoistConstants, const std::string &keyStorage, int c1Cache) {
-        return std::make_unique<B200Server>(params, capacity, device, maxTenants ? *maxTenants : -1, rotationKeys, hoistConstants, keyStorage, c1Cache);
+                       const std::string &hoistConstants, const std::string &keyStorage, int c1Cache, int storeEntries) {
+        return std::make_unique<B200Server>(params, capacity, device, maxTenants ? *maxTenants : -1, rotationKeys, hoistConstants, keyStorage, c1Cache,
+                                            storeEntries);
       }), py::arg("params"), py::arg("capacity") = 64, py::arg("device") = 0, py::arg("max_tenants") = py::none(), py::arg("rotation_keys") = "program",
-      py::arg("hoist_constants") = "stored", py::arg("key_storage") = "expanded", py::arg("c1_cache") = 0,
+      py::arg("hoist_constants") = "stored", py::arg("key_storage") = "expanded", py::arg("c1_cache") = 0, py::arg("store_entries") = 0,
       "capacity: device slots (key-bank regions).  max_tenants None or == capacity: a tenant id is its slot, filled when its keys are "
       "added.  max_tenants > capacity: up to max_tenants tenants' keys in page-locked host memory, paged into the slots (least "
       "recently used first) as batches need them.  rotation_keys: the Galois keys every tenant supplies -- \"program\", one per "
@@ -544,7 +551,8 @@ PYBIND11_MODULE(_eva_b200, m) {
       "half from the seed (same outputs, half the slot; compressed keys only).  c1_cache (key_storage=\"seeded\", 0 <= c1_cache <= "
       "capacity): device regions, each holding the expanded c1 rows of one tenant; the instances of a batch whose tenant holds one read "
       "them instead of drawing (same outputs).  The tenants with the most instances in a batch are admitted first, the least recently "
-      "used region is evicted; tenants without a region draw")
+      "used region is evicted; tenants without a region draw.  store_entries: device entries of the ciphertext store, each holding "
+      "one stored size-2 input ciphertext (store / release; 0: no store)")
       .def("add_raw_keys", [](B200Server &s, const u64arr &relin, const std::map<u64, u64arr> &galois) {
         const std::size_t kk = s.shared()->dev->k(), N = s.shared()->dev->N();
         requireShape(relin, {kk - 1, 2, kk, N}, "relinearization key");
@@ -616,7 +624,12 @@ PYBIND11_MODULE(_eva_b200, m) {
         return s.addKeys(relin.data(), g);
       }, py::arg("public_context"), "add a client's B200Public (same N and primes): compressed (add_compressed_keys) when its keys were "
          "expanded from seeds (generate_keys, or a loaded compressed context), in full (add_raw_keys) otherwise")
-      .def("remove_keys", &B200Server::removeKeys, py::arg("tenant"))
+      .def("remove_keys", &B200Server::removeKeys, py::arg("tenant"), "also releases the tenant's stored ciphertexts")
+      .def("store", &B200Server::store, py::arg("tenant"), py::arg("enc"), py::call_guard<py::gil_scoped_release>(),
+           "keep the ciphertexts of `enc` (B200Public.encrypt or B200Secret.encrypt; every value a ciphertext) on the device as the "
+           "tenant's entries, all or nothing; a seeded one is expanded once here.  Returns {name: handle}: a request names an entry "
+           "with B200Valuation.set_stored(name, handle), and its outputs are those of the same ciphertext sent inline")
+      .def("release", &B200Server::release, py::arg("handle"), "free a stored ciphertext's entry; its handle names nothing afterwards")
       .def("execute", [](B200Server &s, Program &prog, int tenant, const B200Valuation &in) {
         return std::move(s.executeBatch(prog, {{tenant, &in}})[0]);
       }, py::arg("program"), py::arg("tenant"), py::arg("inputs"), py::call_guard<py::gil_scoped_release>())
@@ -669,6 +682,12 @@ PYBIND11_MODULE(_eva_b200, m) {
         d["c1_cached"] = c1 ? c1->cache().cached() : std::vector<int>();
         d["c1_fills"] = c1 ? c1->cache().fills() : 0;
         d["c1_evictions"] = c1 ? c1->cache().evictions() : 0;
+        const CipherStore *st = s.cipherStore();
+        const std::size_t entryBytes = 2 * (std::size_t)(s.shared()->dev->k() - 1) * s.shared()->dev->N() * 8;
+        d["store_entries"] = st ? st->capacity() : 0;
+        d["stored"] = st ? st->used() : 0;
+        d["store_entry_bytes"] = entryBytes;
+        d["store_bytes"] = st ? entryBytes * (std::size_t)st->capacity() : 0;
         return d;
       }, "capacity / device_slots: key-bank regions; rotation_keys: the key set of galois_elements (\"program\" or \"power_of_two\"); "
          "hoist_constants: \"stored\" or \"inline\" (then hoist_const_bytes_per_tenant is 0 and indicator_bytes the one shared copy of "
@@ -677,7 +696,8 @@ PYBIND11_MODULE(_eva_b200, m) {
          "holding a slot; host_key_bytes: page-locked host memory of the paged keys (compressed tenants: c0 rows and seeds); "
          "compressed_tenants: tenants added in compressed form; fills: slots filled (keys uploaded and "
          "constants computed); evictions: resident tenants displaced by a fill; c1_cache: c1 regions (c1_cache_bytes of device memory); "
-         "c1_cached: the tenants holding one; c1_fills: regions expanded; c1_evictions: cached tenants displaced by a fill")
+         "c1_cached: the tenants holding one; c1_fills: regions expanded; c1_evictions: cached tenants displaced by a fill; "
+         "store_entries: entries of the ciphertext store (store_bytes of device memory, store_entry_bytes each); stored: entries in use")
       .def("primes", [](B200Server &s) { return s.shared()->dev->primes(); })
       // ---- benchmark hooks (as B200Public's): device-resident execution of requests staged on a plan replica
       .def("stage_inputs", [](B200Server &s, Program &prog, const Requests &rq, std::uintptr_t stream, int replica) {

@@ -145,6 +145,9 @@ COMPRESSED_RELIN_KEYS, COMPRESSED_GALOIS_KEYS = 16, 17
 # payload kind of a seed-compressed input ciphertext (B200Secret.encrypt), under the CIPHERTEXT object: c0 [ell][N], and in the
 # header's extra words the 32-byte seed of c1 as 4 little-endian u64 words
 COMPRESSED_CIPHERTEXT = 18
+# payload kind of a reference to a ciphertext kept in a B200Server's store, under the CIPHERTEXT object: the store's handle as a
+# one-element u64 array
+STORED_CIPHERTEXT = 19
 
 
 # ------------------------------------------------------------------ Program / parameters / signature
@@ -378,6 +381,9 @@ def valuation_to_msg(val):
         elif kind == "seeded_cipher":
             o = msg.values[name]
             o.seal_type, o.data = CIPHERTEXT, _pack(COMPRESSED_CIPHERTEXT, arr, scale, extra=_seed_words(val.get_seed(name)))
+        elif kind == "stored":
+            o = msg.values[name]
+            o.seal_type, o.data = CIPHERTEXT, _pack(STORED_CIPHERTEXT, np.array([arr], dtype=np.uint64))
         elif kind == "plain":
             o = msg.values[name]
             o.seal_type, o.data = PLAINTEXT, _pack(PLAINTEXT, arr, scale)
@@ -397,6 +403,11 @@ def valuation_from_msg(msg):
             if len(words) != 4:
                 raise RuntimeError("compressed ciphertext %s: the seed must be 32 bytes" % name)
             val.set_seeded_cipher(name, arr, _seed_bytes(words), scale)
+        elif o.seal_type == CIPHERTEXT and _kind(o.data) == STORED_CIPHERTEXT:
+            arr, _, words = _unpack(o.data, STORED_CIPHERTEXT)
+            if arr.shape != (1,) or words:
+                raise RuntimeError("stored ciphertext %s: the payload must be one u64 handle" % name)
+            val.set_stored(name, int(arr[0]))
         elif o.seal_type == CIPHERTEXT:
             arr, scale, _ = _unpack(o.data, CIPHERTEXT)
             val.set_cipher(name, arr, scale)

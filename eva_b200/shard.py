@@ -192,6 +192,9 @@ def _subset(inputs, names):
                 out.set_cipher(name, arr, scale)
             elif kind == "seeded_cipher":      # carried compressed: the instance that stages it expands c1
                 out.set_seeded_cipher(name, arr, inputs.get_seed(name), scale)
+            elif kind == "stored":             # the entry lives in one server's store; a B200Public has none
+                raise ValueError("input %s is a reference to a stored ciphertext (handle %d): the sharded modes run on B200Public "
+                                 "contexts, which have no store; send the ciphertext inline" % (name, arr))
             elif kind == "plain":
                 out.set_plain(name, arr, scale)
             else:

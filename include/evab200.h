@@ -262,6 +262,12 @@ int evab_expand_key_uniform(evab_ctx *ctx, int n, const uint8_t *d_seeds, const 
  * several launches on `stream`).  Stream-ordered, does not synchronise.  1 <= n <= 65535, 1 <= h_ell[i] <= k-1. */
 int evab_expand_cipher_uniform(evab_ctx *ctx, int n, const uint8_t *h_seeds, uint64_t *const *h_c1, const int *h_ell, const uint64_t *h_moduli,
                                void *stream);
+/* Server-resident ciphertexts: copy n device ranges, entry i the h_words[i] words at h_src[i] to h_dst[i] (device pointers, both
+ * 16-byte aligned; h_words[i] even; the ranges of one call must not overlap a destination).  Nothing else is written.  The host
+ * tables are read during the call (the entries travel in the launch arguments, up to 160 per launch; larger n is split into
+ * several launches on `stream`), so a captured graph replays the copies as they were.  Stream-ordered, does not synchronise;
+ * evab_set_batch does not apply.  n >= 0 (0: no launch); the tables must not be null. */
+int evab_gather_ciphers(evab_ctx *ctx, int n, const uint64_t *const *h_src, uint64_t *const *h_dst, const uint64_t *h_words, void *stream);
 /* n <= 16 rotations of ONE ciphertext (seal::Evaluator::rotate_vector, seal_executor.h:176-189) in three kernel launches instead of
  * 3 n: d_out [n][2][ell][N], rotation i by galois_elts[i]; same bits as n calls of evab_rotate_modup_prepared.  d_ext, keys, cadds as there. */
 /* evab_rotate_modup_many and evab_lazy_rotsum read P * c0 from the diagonal of d_ext (ext[m][J] has no entry for m = q_J): call this once
