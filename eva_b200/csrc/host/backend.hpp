@@ -71,26 +71,73 @@ public:
   std::map<std::string, SchemeValue> values;
 };
 
-// Paging of evaluation keys (B200Server with more tenants than key-bank regions): every registered tenant's keys live in a
-// page-locked host block (in full, or compressed: c0 rows and seeds, expanded on the device at every fill), and the bank's regions are device slots holding the keys of the tenants used recently (SlotCache).
-// A batch's missing tenants are filled on the pager's own stream: a fill waits for the runs that may still read its slot (one
-// reader event per slot and replica stream), uploads the keys, recomputes the slot's hoist constants and records the slot's fill
-// event, which every run that reads the slot waits for.  The host never blocks on the way.
-class KeyPager {
+// Ordering of device regions that a fill stream rewrites while runs on other streams read them: a fill waits for the runs that
+// may still read its region (one reader event per region and reader stream), and records the region's fill event, which every run
+// that reads the region waits for.  The host never blocks on the way.
+class RegionFences {
 public:
-  KeyPager(std::shared_ptr<Device> dev, KeyBank &bank, int maxTenants)
-      : dev_(std::move(dev)), bank_(bank), cache_(bank.capacity()), host_(maxTenants), fillEv_(bank.capacity(), nullptr), readers_(bank.capacity()) {
+  RegionFences(std::shared_ptr<Device> dev, int regions) : dev_(std::move(dev)), fillEv_(regions, nullptr), readers_(regions) {
     check(evab_stream_create(dev_->ctx(), &stream_));
   }
-  ~KeyPager() {
+  ~RegionFences() {
     evab_ctx *c = dev_->ctx();
-    evab_sync(c, stream_);   // fills still reading the host blocks
-    for (Block &h : host_) if (h.p) evab_host_free(h.p);
+    evab_sync(c, stream_);
     for (void *e : fillEv_) if (e) evab_event_destroy(c, e);
     for (auto &m : readers_) for (auto &r : m) evab_event_destroy(c, r.second);
     evab_stream_destroy(c, stream_);
   }
-  KeyPager(const KeyPager &) = delete;
+  RegionFences(const RegionFences &) = delete;
+  // the fill stream
+  void *stream() const { return stream_; }
+  // the fill stream waits for every run recorded as a reader of region r
+  void awaitReaders(int r) {
+    for (auto &e : readers_[r]) check(evab_stream_wait_event(dev_->ctx(), stream_, e.second));
+  }
+  // a fill of region r has been enqueued on the fill stream
+  void filled(int r) {
+    if (!fillEv_[r]) check(evab_event_create(dev_->ctx(), &fillEv_[r]));
+    check(evab_event_record(dev_->ctx(), fillEv_[r], stream_));
+  }
+  // the event of the last fill of region r (null: never filled)
+  void *fillEvent(int r) const { return fillEv_[r]; }
+  // a run on `stream` that reads the regions of `entries` (entry e >= 0: region e - base; e < 0: none) waits for their fills; once
+  // enqueued, it is recorded as their reader on that stream
+  void beforeRun(void *stream, const int *entries, int n, int base = 0) {
+    for (int i = 0; i < n; i++)
+      if (firstOf(entries, i))
+        if (void *ev = fillEv_[entries[i] - base]) check(evab_stream_wait_event(dev_->ctx(), stream, ev));
+  }
+  void afterRun(void *stream, const int *entries, int n, int base = 0) {
+    for (int i = 0; i < n; i++) {
+      if (!firstOf(entries, i)) continue;
+      void *&ev = readers_[entries[i] - base][stream];
+      if (!ev) check(evab_event_create(dev_->ctx(), &ev));
+      check(evab_event_record(dev_->ctx(), ev, stream));
+    }
+  }
+
+private:
+  // entries[i] names a region that entries[0 .. i) does not
+  static bool firstOf(const int *entries, int i) { return entries[i] >= 0 && std::find(entries, entries + i, entries[i]) == entries + i; }
+  std::shared_ptr<Device> dev_;
+  std::vector<void *> fillEv_;                      // region -> event of its last fill
+  std::vector<std::map<void *, void *>> readers_;   // region -> (reader stream -> event after its last run that read the region)
+  void *stream_ = nullptr;                          // fills
+};
+
+// Paging of evaluation keys (B200Server with more tenants than key-bank regions): every registered tenant's keys live in a
+// page-locked host block (in full, or compressed: c0 rows and seeds, expanded on the device at every fill), and the bank's regions
+// are device slots holding the keys of the tenants used recently (RegionCache::assignAll).  A batch's missing tenants are filled on
+// the pager's fill stream, ordered against the runs by the slots' RegionFences: a fill uploads the keys and recomputes the slot's
+// hoist constants.
+class KeyPager {
+public:
+  KeyPager(std::shared_ptr<Device> dev, KeyBank &bank, int maxTenants)
+      : dev_(std::move(dev)), bank_(bank), cache_(bank.capacity()), host_(maxTenants), fences_(dev_, bank.capacity()) {}
+  ~KeyPager() {
+    evab_sync(dev_->ctx(), fences_.stream());   // fills still reading the host blocks (fences_ is destroyed after this body)
+    for (Block &h : host_) if (h.p) evab_host_free(h.p);
+  }
   int maxTenants() const { return (int)host_.size(); }
   int tenants() const { return (int)std::count_if(host_.begin(), host_.end(), [](const Block &h) { return h.p != nullptr; }); }
   int compressedTenants() const { return (int)std::count_if(host_.begin(), host_.end(), [](const Block &h) { return h.p && h.compressed; }); }
@@ -117,41 +164,29 @@ public:
   void remove(int t) {
     requireRegistered(t);
     cache_.drop(t);
-    check(evab_sync(dev_->ctx(), stream_));   // a fill may still be reading the block
+    check(evab_sync(dev_->ctx(), fences_.stream()));   // a fill may still be reading the block
     evab_host_free(host_[t].p);
     host_[t] = Block();
   }
   // the slot of every instance of a batch; the missing tenants' fills are enqueued on the pager's stream
   std::vector<int> resolve(const std::vector<int> &tenants) {
-    evab_ctx *c = dev_->ctx();
-    std::vector<SlotCache::Fill> fills;
-    std::vector<int> slots = cache_.assign(tenants, fills);
+    std::vector<RegionCache::Fill> fills;
+    std::vector<int> slots = cache_.assignAll(tenants, fills);
     for (auto &f : fills) {
-      for (auto &r : readers_[f.slot]) check(evab_stream_wait_event(c, stream_, r.second));
+      fences_.awaitReaders(f.region);
       const Block &b = host_[f.tenant];
-      if (b.compressed) bank_.fillCompressed(f.slot, b.p, stream_);
-      else bank_.fill(f.slot, b.p, stream_);
-      if (!fillEv_[f.slot]) check(evab_event_create(c, &fillEv_[f.slot]));
-      check(evab_event_record(c, fillEv_[f.slot], stream_));
+      if (b.compressed) bank_.fillCompressed(f.region, b.p, fences_.stream());
+      else bank_.fill(f.region, b.p, fences_.stream());
+      fences_.filled(f.region);
     }
     return slots;
   }
   // a run on `stream` that reads `slots` waits for their fills; once enqueued, it is recorded as their reader on that stream
-  void beforeRun(void *stream, const int *slots, int n) {
-    for (int i = 0; i < n; i++)
-      if (std::find(slots, slots + i, slots[i]) == slots + i && fillEv_[slots[i]]) check(evab_stream_wait_event(dev_->ctx(), stream, fillEv_[slots[i]]));
-  }
-  void afterRun(void *stream, const int *slots, int n) {
-    for (int i = 0; i < n; i++) {
-      if (std::find(slots, slots + i, slots[i]) != slots + i) continue;
-      void *&ev = readers_[slots[i]][stream];
-      if (!ev) check(evab_event_create(dev_->ctx(), &ev));
-      check(evab_event_record(dev_->ctx(), ev, stream));
-    }
-  }
-  const SlotCache &cache() const { return cache_; }
+  void beforeRun(void *stream, const int *slots, int n) { fences_.beforeRun(stream, slots, n); }
+  void afterRun(void *stream, const int *slots, int n) { fences_.afterRun(stream, slots, n); }
+  const RegionCache &cache() const { return cache_; }
   // the event of the last fill of a slot (null: never filled by the pager)
-  void *fillEvent(int slot) const { return fillEv_[slot]; }
+  void *fillEvent(int slot) const { return fences_.fillEvent(slot); }
   std::size_t hostBytes() const {
     std::size_t w = 0;
     for (const Block &b : host_) w += b.words;
@@ -173,97 +208,60 @@ private:
   }
   std::shared_ptr<Device> dev_;
   KeyBank &bank_;
-  SlotCache cache_;
+  RegionCache cache_;
   std::vector<Block> host_;                         // tenant -> page-locked keys
-  std::vector<void *> fillEv_;                      // slot -> event of its last fill
-  std::vector<std::map<void *, void *>> readers_;   // slot -> (replica stream -> event after its last run that read the slot)
-  void *stream_ = nullptr;                          // fills
+  RegionFences fences_;                             // of the slots
 };
 
-// Cached c1 rows of a seeded key bank (B200Server c1_cache): C1Cache decides which tenants hold the bank's c1 regions, and a fill
-// expands a tenant's c1 rows from the seeds in its bank slot (KeyBank::fillC1) on the store's own stream.  A fill waits for the
-// fill of the tenant's slot (paging: its images must be there) and for the runs that may still read the region (one reader event
-// per region and replica stream), and records the region's fill event, which every run that reads the region waits for.  The rows
-// depend on the seeds only, so a tenant keeps its region while its slot is paged out and back in; removing its keys drops it.
+// Cached c1 rows of a seeded key bank (B200Server c1_cache): RegionCache::assignByCount decides which tenants hold the bank's c1
+// regions, and a fill expands a tenant's c1 rows from the seeds in its bank slot (KeyBank::fillC1) on the store's fill stream,
+// ordered against the runs by the regions' RegionFences.  A fill also waits for the fill of the tenant's slot (paging: its images
+// must be there).  The rows depend on the seeds only, so a tenant keeps its region while its slot is paged out and back in;
+// removing its keys drops it.
 class C1Store {
 public:
   C1Store(std::shared_ptr<Device> dev, KeyBank &bank, KeyPager *pager)
-      : dev_(std::move(dev)), bank_(bank), pager_(pager), cache_(bank.c1Regions()), fillEv_(bank.c1Regions(), nullptr), readers_(bank.c1Regions()) {
-    check(evab_stream_create(dev_->ctx(), &stream_));
-  }
-  ~C1Store() {
-    evab_ctx *c = dev_->ctx();
-    evab_sync(c, stream_);
-    for (void *e : fillEv_) if (e) evab_event_destroy(c, e);
-    for (auto &m : readers_) for (auto &r : m) evab_event_destroy(c, r.second);
-    evab_stream_destroy(c, stream_);
-  }
-  C1Store(const C1Store &) = delete;
+      : dev_(std::move(dev)), bank_(bank), pager_(pager), cache_(bank.c1Regions()), fences_(dev_, bank.c1Regions()) {}
   // the c1 table entry of every instance of a batch (bank region capacity + h, or -1: draws) whose instances hold bank slots
   // `slots`; the admitted missing tenants' fills are enqueued on the store's stream
   std::vector<int> resolve(const std::vector<int> &tenants, const std::vector<int> &slots) {
-    evab_ctx *c = dev_->ctx();
-    std::vector<C1Cache::Fill> fills;
-    std::vector<int> regions = cache_.assign(tenants, fills);
+    std::vector<RegionCache::Fill> fills;
+    std::vector<int> regions = cache_.assignByCount(tenants, fills);
     for (auto &f : fills) {
       const int slot = slots[std::find(tenants.begin(), tenants.end(), f.tenant) - tenants.begin()];
-      for (auto &r : readers_[f.region]) check(evab_stream_wait_event(c, stream_, r.second));
-      if (pager_) if (void *ev = pager_->fillEvent(slot)) check(evab_stream_wait_event(c, stream_, ev));
-      bank_.fillC1(f.region, slot, stream_);
-      if (!fillEv_[f.region]) check(evab_event_create(c, &fillEv_[f.region]));
-      check(evab_event_record(c, fillEv_[f.region], stream_));
+      fences_.awaitReaders(f.region);
+      if (pager_) if (void *ev = pager_->fillEvent(slot)) check(evab_stream_wait_event(dev_->ctx(), fences_.stream(), ev));
+      bank_.fillC1(f.region, slot, fences_.stream());
+      fences_.filled(f.region);
     }
     for (int &r : regions) if (r >= 0) r += bank_.capacity();
     return regions;
   }
   // a run on `stream` with c1 table entries `rows` waits for their regions' fills; once enqueued, it is recorded as their reader
-  void beforeRun(void *stream, const int *rows, int n) {
-    for (int i = 0; i < n; i++)
-      if (rows[i] >= 0 && std::find(rows, rows + i, rows[i]) == rows + i) {
-        if (void *ev = fillEv_[rows[i] - bank_.capacity()]) check(evab_stream_wait_event(dev_->ctx(), stream, ev));
-      }
-  }
-  void afterRun(void *stream, const int *rows, int n) {
-    for (int i = 0; i < n; i++) {
-      if (rows[i] < 0 || std::find(rows, rows + i, rows[i]) != rows + i) continue;
-      void *&ev = readers_[rows[i] - bank_.capacity()][stream];
-      if (!ev) check(evab_event_create(dev_->ctx(), &ev));
-      check(evab_event_record(dev_->ctx(), ev, stream));
-    }
-  }
+  void beforeRun(void *stream, const int *rows, int n) { fences_.beforeRun(stream, rows, n, bank_.capacity()); }
+  void afterRun(void *stream, const int *rows, int n) { fences_.afterRun(stream, rows, n, bank_.capacity()); }
   void drop(int tenant) { cache_.drop(tenant); }
-  const C1Cache &cache() const { return cache_; }
+  const RegionCache &cache() const { return cache_; }
 
 private:
   std::shared_ptr<Device> dev_;
   KeyBank &bank_;
   KeyPager *pager_;
-  C1Cache cache_;
-  std::vector<void *> fillEv_;                      // region -> event of its last fill
-  std::vector<std::map<void *, void *>> readers_;   // region -> (replica stream -> event after its last run that read the region)
-  void *stream_ = nullptr;                          // fills
+  RegionCache cache_;
+  RegionFences fences_;   // of the c1 regions
 };
 
 // Server-resident input ciphertexts (B200Server store_entries): one device allocation of `capacity` entries of 2 (k-1) N words,
 // each holding one tenant's size-2 ciphertext [2][ell][N] at its level.  A request names an entry by handle where it would carry
 // the ciphertext, and staging copies the entry into the arena (evab_gather_ciphers).  Handles increase and are never reused, so a
 // released handle, or one of a tenant whose keys were removed (its entries go with them), names nothing afterwards.  Entries do
-// not depend on key residency.  A fill runs on the store's own stream and is synchronised before store() returns; it first waits
-// for the gathers that may still read a released entry (one event per staging stream, recorded after its last gather).
+// not depend on key residency.  A fill runs on the store's fill stream and is synchronised before store() returns; it first waits
+// for the gathers that may still read a released entry (the whole store is one region of its RegionFences, read by every gather).
 class CipherStore {
 public:
   struct Entry { int tenant = -1, ell = 0; double scale = 0; std::uint64_t handle = 0; };   // handle 0: free
   CipherStore(std::shared_ptr<Device> dev, int capacity)
-      : dev_(std::move(dev)), entries_(capacity), words_(dev_, (std::size_t)capacity * entryWords()) {
-    check(evab_stream_create(dev_->ctx(), &stream_));
-  }
-  ~CipherStore() {
-    evab_ctx *c = dev_->ctx();
-    evab_sync(c, stream_);
-    for (auto &e : gatherEv_) evab_event_destroy(c, e.second);
-    evab_stream_destroy(c, stream_);
-  }
-  CipherStore(const CipherStore &) = delete;
+      : dev_(std::move(dev)), entries_(capacity), words_(dev_, (std::size_t)capacity * entryWords()), fences_(dev_, 1) {}
   int capacity() const { return (int)entries_.size(); }
   int used() const { return (int)slotOf_.size(); }
   std::size_t entryWords() const { return 2 * (std::size_t)(dev_->k() - 1) * dev_->N(); }
@@ -288,8 +286,8 @@ public:
     if (capacity() - used() < (int)v.size())
       throw std::invalid_argument("the ciphertext store has " + std::to_string(capacity() - used()) + " free entries of store_entries=" +
                                   std::to_string(capacity()) + " and the valuation holds " + std::to_string(v.size()) + ": release entries first");
-    evab_ctx *c = dev_->ctx();
-    for (auto &e : gatherEv_) check(evab_stream_wait_event(c, stream_, e.second));
+    void *stream = fences_.stream();
+    fences_.awaitReaders(0);
     std::vector<int> slots;
     for (int i = 0; i < capacity() && slots.size() < v.size(); i++) if (!entries_[i].handle) slots.push_back(i);
     std::vector<KeySeed> seeds;
@@ -299,15 +297,15 @@ public:
     for (auto &kv : v) {
       u64 *dst = words_.get() + slots[i++] * entryWords();
       if (auto *hc = std::get_if<HostCipher>(&kv.second)) {
-        dev_->upload(dst, hc->data.data(), hc->data.size() * 8, stream_);
+        dev_->upload(dst, hc->data.data(), hc->data.size() * 8, stream);
       } else {
         auto &sc = std::get<HostSeededCipher>(kv.second);
-        dev_->upload(dst, sc.c0.data(), sc.c0.size() * 8, stream_);
+        dev_->upload(dst, sc.c0.data(), sc.c0.size() * 8, stream);
         seeds.push_back(sc.seed); c1.push_back(dst + sc.c0.size()); ells.push_back(sc.ell);
       }
     }
-    if (!seeds.empty()) expandCiphers(*dev_, (int)seeds.size(), seeds.data(), c1.data(), ells.data(), stream_);
-    check(evab_sync(c, stream_));   // the first request that names an entry needs no event
+    if (!seeds.empty()) expandCiphers(*dev_, (int)seeds.size(), seeds.data(), c1.data(), ells.data(), stream);
+    check(evab_sync(dev_->ctx(), stream));   // the first request that names an entry needs no fill event
     std::map<std::string, std::uint64_t> out;
     i = 0;
     for (auto &kv : v) {
@@ -340,19 +338,23 @@ public:
   }
   // `stream` has enqueued gathers from the store: a later fill waits for them
   void afterGather(void *stream) {
-    void *&ev = gatherEv_[stream];
-    if (!ev) check(evab_event_create(dev_->ctx(), &ev));
-    check(evab_event_record(dev_->ctx(), ev, stream));
+    const int store = 0;
+    fences_.afterRun(stream, &store, 1);
   }
 
 private:
   std::shared_ptr<Device> dev_;
   std::vector<Entry> entries_;
   DBuf words_;                                      // [capacity][2 (k-1) N]
+  RegionFences fences_;                             // region 0: words_ (destroyed first: its fills write words_)
   std::map<std::uint64_t, int> slotOf_;             // live handle -> entry
-  std::map<void *, void *> gatherEv_;               // staging stream -> event after its last gather
-  void *stream_ = nullptr;                          // fills
   std::uint64_t next_ = 1;
+};
+
+// where every instance of a batch reads its keys: its key-bank slot (empty: no key bank) and its c1 table entry (empty: no c1 cache)
+struct Residency {
+  std::vector<int> slots, c1;
+  const int *c1At(int b0) const { return c1.empty() ? nullptr : c1.data() + b0; }
 };
 
 struct Shared {
@@ -365,10 +367,22 @@ struct Shared {
   std::unique_ptr<CipherStore> store;   // B200Server with store_entries > 0: the tenants' stored input ciphertexts
   std::mutex execMutex;   // serialises execute / executeMany callers of one context (see executeMany), and key-bank changes
   void requireTenant(int t) const { if (pager) pager->requireRegistered(t); else bank->requireOccupied(t); }
-  // the bank region of every instance (with paging: resolved, and missing tenants' fills enqueued)
-  std::vector<int> slotsFor(const std::vector<int> &tenants) { return pager ? pager->resolve(tenants) : tenants; }
-  // the c1 table entry of every instance (with a c1 cache: resolved, and admitted tenants' fills enqueued; else empty)
-  std::vector<int> c1For(const std::vector<int> &tenants, const std::vector<int> &slots) { return c1 ? c1->resolve(tenants, slots) : std::vector<int>(); }
+  // the residency of every instance (with paging and a c1 cache: resolved, and the missing tenants' fills enqueued, slots first)
+  Residency resolve(const std::vector<int> &tenants) {
+    Residency r;
+    r.slots = pager ? pager->resolve(tenants) : tenants;
+    if (c1) r.c1 = c1->resolve(tenants, r.slots);
+    return r;
+  }
+  // a run on `stream` of instances b0 .. b0 + nb waits for the fills of what they read; once enqueued, it is recorded as its reader
+  void beforeRun(void *stream, const Residency &r, int b0, int nb) {
+    if (pager) pager->beforeRun(stream, r.slots.data() + b0, nb);
+    if (c1) c1->beforeRun(stream, r.c1.data() + b0, nb);
+  }
+  void afterRun(void *stream, const Residency &r, int b0, int nb) {
+    if (pager) pager->afterRun(stream, r.slots.data() + b0, nb);
+    if (c1) c1->afterRun(stream, r.c1.data() + b0, nb);
+  }
 };
 
 // SEALPublic::encrypt's checks, slot replication and encoding (reference eva/seal/seal.cpp:24-102), shared by the public-key
@@ -651,11 +665,8 @@ public:
       checkStored(first, program, inputs.data(), p.tenants.empty() ? nullptr : p.tenants.data(), B);
     }
     std::vector<char> busy(R, 0);
-    // key-bank region of every instance, resolved at every enqueue (so that collect's redo refills a tenant evicted meanwhile)
-    const std::vector<int> slots = p.tenants.empty() ? std::vector<int>() : s_->slotsFor(p.tenants);
-    const std::vector<int> c1 = p.tenants.empty() ? std::vector<int>() : s_->c1For(p.tenants, slots);
-    KeyPager *pager = s_->pager.get();
-    C1Store *c1s = s_->c1.get();
+    // residency of every instance, resolved at every enqueue (so that collect's redo refills a tenant evicted meanwhile)
+    const Residency res = s_->resolve(p.tenants);
     for (int b0 = 0, g = 0; b0 < B; b0 += F, g++) {
       const int nb = std::min(F, B - b0);
       const int r = g % R;
@@ -665,18 +676,15 @@ public:
       void *st = ex.mainStream();
       if (busy[r]) s_->dev->sync(st);   // the replica's arena is reused: wait for its previous chunk
       busy[r] = 1;
-      if (!slots.empty()) ex.setTenants(slots.data() + b0, nb);
-      if (!c1.empty()) ex.setC1Rows(c1.data() + b0, nb);
+      if (!res.slots.empty()) ex.setKeyTable(res.slots.data() + b0, res.c1At(b0), nb);
       if (std::find(streams.begin(), streams.end(), st) == streams.end()) streams.push_back(st);
       if (std::find(p.plans.begin(), p.plans.end(), holder) == p.plans.end()) p.plans.push_back(holder);
       auto t1 = now();
       stageInputs(ex, program, inputs.data() + b0, nb, st);
       auto t2 = now();
-      if (pager) pager->beforeRun(st, slots.data() + b0, nb);
-      if (c1s) c1s->beforeRun(st, c1.data() + b0, nb);
+      s_->beforeRun(st, res, b0, nb);
       ex.run(st);
-      if (pager) pager->afterRun(st, slots.data() + b0, nb);
-      if (c1s) c1s->afterRun(st, c1.data() + b0, nb);
+      s_->afterRun(st, res, b0, nb);
       auto t3 = now();
       tPlan += std::chrono::duration<double>(t1 - t0).count(); tStage += std::chrono::duration<double>(t2 - t1).count();
       tRun += std::chrono::duration<double>(t3 - t2).count();
@@ -818,8 +826,7 @@ public:
     for (auto &r : rq) in.push_back(r.second);
     pub_->checkStored(ex, prog, in.data(), tenants.data(), (int)in.size());
     staged_[&ex] = tenants;
-    const std::vector<int> slots = shared()->slotsFor(tenants);
-    setSlots(ex, slots, shared()->c1For(tenants, slots), stream);
+    setKeyTable(ex, shared()->resolve(tenants), stream);
     pub_->stageInputs(ex, prog, in.data(), (int)in.size(), stream);
   }
   // tenants: replaces the staged tenants of the replica (same count)
@@ -836,14 +843,11 @@ public:
     if (!pager && it == staged_.end()) { ex.run(stream); return; }
     if (it == staged_.end()) throw std::runtime_error("run_resident: stage the replica's inputs first");
     if (pager) for (int t : it->second) pager->requireRegistered(t);
-    const std::vector<int> slots = shared()->slotsFor(it->second);
-    const std::vector<int> c1 = shared()->c1For(it->second, slots);
-    setSlots(ex, slots, c1, stream);
-    if (pager) pager->beforeRun(stream, slots.data(), batch);
-    if (!c1.empty()) shared()->c1->beforeRun(stream, c1.data(), batch);
+    const Residency res = shared()->resolve(it->second);
+    setKeyTable(ex, res, stream);
+    shared()->beforeRun(stream, res, 0, batch);
     ex.run(stream);
-    if (pager) pager->afterRun(stream, slots.data(), batch);
-    if (!c1.empty()) shared()->c1->afterRun(stream, c1.data(), batch);
+    shared()->afterRun(stream, res, 0, batch);
   }
   std::shared_ptr<PendingBatch> submit(Program &program, const std::vector<std::pair<int, const B200Valuation *>> &requests, int slot = 0) {
     std::vector<const B200Valuation *> in;
@@ -863,16 +867,15 @@ public:
   std::shared_ptr<Shared> shared() const { return pub_->shared(); }
 
 private:
-  // the executor's page-locked tenant and c1 tables are read by its previous run's stream-ordered uploads: rewritten only after that
-  // run (c1 empty: no c1 cache)
   void requireStore() const {
     if (!shared()->store) throw std::invalid_argument("this server has no ciphertext store: build it with store_entries > 0");
   }
-  void setSlots(Executor &ex, const std::vector<int> &slots, const std::vector<int> &c1, void *stream) {
-    if (ex.tenantsAre(slots.data(), (int)slots.size()) && (c1.empty() || ex.c1RowsAre(c1.data(), (int)c1.size()))) return;
+  // the executor's page-locked key table is read by its previous run's stream-ordered upload: rewritten only after that run
+  void setKeyTable(Executor &ex, const Residency &res, void *stream) {
+    const int n = (int)res.slots.size();
+    if (ex.keyTableIs(res.slots.data(), res.c1At(0), n)) return;
     shared()->dev->sync(stream);
-    ex.setTenants(slots.data(), (int)slots.size());
-    if (!c1.empty()) ex.setC1Rows(c1.data(), (int)c1.size());
+    ex.setKeyTable(res.slots.data(), res.c1At(0), n);
   }
   std::string rotationKeys_, hoistConstants_, keyStorage_;
   std::unique_ptr<B200Public> pub_;

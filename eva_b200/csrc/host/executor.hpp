@@ -227,7 +227,7 @@ private:
 
 class Executor {
 public:
-  // bank != null: keys come from the bank, tenant per instance (setTenants); `keys` is not read.  The plan is the same either way.
+  // bank != null: keys come from the bank, tenant per instance (setKeyTable); `keys` is not read.  The plan is the same either way.
   Executor(std::shared_ptr<Device> dev, const KeySet &keys, Program &program, ExecOptions opt = {}, const KeyBank *bank = nullptr)
       : dev_(std::move(dev)), keys_(keys), bank_(bank), prog_(program), plan_(plan(opt)), N_(dev_->N()) {
     materialise();
@@ -235,8 +235,7 @@ public:
   ~Executor() {
     if (graph_) evab_graph_destroy(dev_->ctx(), graph_);
     if (hostFlags_) evab_host_free(hostFlags_);
-    if (tenantHost_) evab_host_free(tenantHost_);
-    if (c1Host_) evab_host_free(c1Host_);
+    if (keyTableHost_) evab_host_free(keyTableHost_);
     for (void *e : events_) evab_event_destroy(dev_->ctx(), e);
     for (void *s : streams_) evab_stream_destroy(dev_->ctx(), s);
   }
@@ -264,24 +263,22 @@ public:
   // device-resident run: inputs must already be in valuePtr(input term); raw
   // inputs set through setRawInput.  Enqueues the whole program on `stream`
   // (graph launch or multi-stream replay); does not synchronise.
-  // the tenant of every instance of the next runs (bank-bound executors).  The page-locked copy is read by run()'s stream-ordered
-  // upload: callers rewrite it only once the previous run's stream has been synchronised
-  void setTenants(const int *tenants, int n) {
-    if (!bank_ || n != plan_.opt.batch) throw std::logic_error("setTenants: one tenant per instance of a bank-bound plan");
-    for (int b = 0; b < n; b++) tenantHost_[b] = tenants[b];
+  // the key table of the next runs (bank-bound executors): the bank slot of every instance, then, for a bank with c1 regions, its
+  // c1 table entry, capacity + h or -1 (draws); c1 is null exactly when the bank has no c1 regions.  The page-locked copy is read
+  // by run()'s stream-ordered upload: callers rewrite it only once the previous run's stream has been synchronised
+  void setKeyTable(const int *slots, const int *c1, int n) {
+    if (!bank_ || n != plan_.opt.batch || !c1 != !c1Table())
+      throw std::logic_error("setKeyTable: one slot per instance of a bank-bound plan, and c1 entries exactly when the bank has c1 regions");
+    std::copy(slots, slots + n, keyTableHost_);
+    if (c1) std::copy(c1, c1 + n, keyTableHost_ + n);
   }
-  bool tenantsAre(const int *tenants, int n) const { return bank_ && n == plan_.opt.batch && std::equal(tenants, tenants + n, tenantHost_); }
-  // the c1 table entry of every instance of the next runs (banks with c1 regions): capacity + h, or -1 (draws).  Rewritten under the
-  // same rule as the tenant table
-  void setC1Rows(const int *regions, int n) {
-    if (!c1Host_ || n != plan_.opt.batch) throw std::logic_error("setC1Rows: one entry per instance of a plan bound to a bank with c1 regions");
-    for (int b = 0; b < n; b++) c1Host_[b] = regions[b];
+  bool keyTableIs(const int *slots, const int *c1, int n) const {
+    return bank_ && n == plan_.opt.batch && !c1 == !c1Table() && std::equal(slots, slots + n, keyTableHost_) &&
+           (!c1 || std::equal(c1, c1 + n, keyTableHost_ + n));
   }
-  bool c1RowsAre(const int *regions, int n) const { return c1Host_ && n == plan_.opt.batch && std::equal(regions, regions + n, c1Host_); }
   void run(void *stream) {
     if (rawDirty_) { evalRawAndEncodes(stream); rawDirty_ = false; }
-    if (bank_) dev_->upload(tenantDev_.get(), tenantHost_, 4 * (std::size_t)plan_.opt.batch, stream);   // read by the kernels, not baked into the graph
-    if (c1Host_) dev_->upload(c1Dev_.get(), c1Host_, 4 * (std::size_t)plan_.opt.batch, stream);
+    if (bank_) dev_->upload(keyTableDev_.get(), keyTableHost_, 4 * keyTableEntries(), stream);   // read by the kernels, not baked into the graph
     if (plan_.opt.useGraph && verbosity() < 2) {   // debug verbosity: step-by-step replay so that every term is reported
       if (!graph_ || !graphValid_) capture();
       check(evab_graph_launch(dev_->ctx(), graph_, stream));
@@ -359,17 +356,15 @@ private:
     });
     if (p.numFlags) check(evab_host_alloc(8 * p.numFlags * 8 * (std::size_t)B, (void **)&hostFlags_));
     if (bank_) {
-      tenantDev_ = DBuf(dev_, ((std::size_t)B + 1) / 2);
-      check(evab_host_alloc(4 * (std::size_t)B, (void **)&tenantHost_));
-      std::fill(tenantHost_, tenantHost_ + B, 0);
-      if (bank_->c1Regions()) {
-        c1Dev_ = DBuf(dev_, ((std::size_t)B + 1) / 2);
-        check(evab_host_alloc(4 * (std::size_t)B, (void **)&c1Host_));
-        std::fill(c1Host_, c1Host_ + B, -1);
-      }
+      keyTableDev_ = DBuf(dev_, (keyTableEntries() + 1) / 2);
+      check(evab_host_alloc(4 * keyTableEntries(), (void **)&keyTableHost_));
+      std::fill(keyTableHost_, keyTableHost_ + B, 0);
+      std::fill(keyTableHost_ + B, keyTableHost_ + keyTableEntries(), -1);
       dev_->sync();
     }
   }
+  bool c1Table() const { return bank_ && bank_->c1Regions() > 0; }
+  std::size_t keyTableEntries() const { return (std::size_t)plan_.opt.batch * (c1Table() ? 2 : 1); }
   const u64 *relinKey() const { return bank_ ? bank_->relin() : keys_.relin.get(); }
   const u64 *galoisKey(u64 elt) const { return bank_ ? bank_->galois(elt) : keys_.galois.at(elt).get(); }
   // a hoisted rotation's constant operand: cadd_g at level ell, or with inline constants the element's indicator rows
@@ -590,10 +585,11 @@ private:
     const Plan &p = plan_;
     evab_ctx *c = dev_->ctx();
     BatchGuard bg(p.opt.batch, p.stride, p.rawStride);
-    KeyBankGuard kg(bank_ ? reinterpret_cast<const std::int32_t *>(tenantDev_.get()) : nullptr, bank_ ? bank_->stride() : 0);
+    const std::int32_t *table = bank_ ? reinterpret_cast<const std::int32_t *>(keyTableDev_.get()) : nullptr;
+    KeyBankGuard kg(table, bank_ ? bank_->stride() : 0);
     HoistInlineGuard hg(bank_ && bank_->inlineConstants());
     KeySeededGuard sg(bank_ && bank_->seededKeys());
-    KeyC1Guard cg(c1Host_ ? reinterpret_cast<const std::int32_t *>(c1Dev_.get()) : nullptr);
+    KeyC1Guard cg(c1Table() ? table + p.opt.batch : nullptr);
     void *forkEv = events_[p.numEvents + p.usedStreams];
     for (int b = 0; p.numFlags && b < p.opt.batch; b++)   // zero-coefficient flags of the shared mod-ups
       check(evab_memset_zero(c, arena_.get() + (std::size_t)b * p.stride + p.flagsOff, 8 * p.numFlags * 8, stream));
@@ -629,10 +625,8 @@ private:
   std::vector<std::vector<std::vector<double>>> rawsB_;   // [instance][term]
   std::map<std::pair<u64, int>, DBuf> hoistConst_;        // (galois element, ell) -> cadd [2][ell+1][N]
   u64 *hostFlags_ = nullptr;                              // page-locked copy of the flags of the last run
-  DBuf tenantDev_;                                        // bank-bound: int32 tenant of every instance, read by the kernels
-  std::int32_t *tenantHost_ = nullptr;                    // its page-locked source (setTenants)
-  DBuf c1Dev_;                                            // bank with c1 regions: int32 c1 table entry of every instance
-  std::int32_t *c1Host_ = nullptr;                        // its page-locked source (setC1Rows)
+  DBuf keyTableDev_;                                      // bank-bound: int32 [batch] slots, then [batch] c1 entries (c1Table), read by the kernels
+  std::int32_t *keyTableHost_ = nullptr;                  // its page-locked source (setKeyTable)
   std::unordered_set<std::uint64_t> rawUploaded_;
   bool staticEncoded_ = false;
   DBuf rawArena_;

@@ -170,11 +170,12 @@ PYBIND11_MODULE(_eva_b200, m) {
     PackResult r = packArena(ps, pb);
     return py::make_tuple(r.offsets, r.waits, r.peak);
   }, py::arg("steps"), py::arg("buffers"));
-  // test hook: the key pager's residency policy alone (host/slot_cache.hpp).  Replays batches of tenant ids through a cache of
-  // `slots` slots; an entry ("remove", t) drops tenant t instead.  Returns (per entry: (slots of the instances, [(tenant, slot,
-  // evicted or -1)]), the error message, or None for a removal; fills; evictions)
-  m.def("_slot_cache", [](int slots, const std::vector<py::object> &ops) {
-    SlotCache c(slots);
+  // test hooks: a residency policy alone (host/slot_cache.hpp).  Replay batches of tenant ids through a cache of `regions` regions;
+  // an entry ("remove", t) drops tenant t instead.  Return (per entry: the region of every instance (-1: draws) and [(tenant,
+  // region, evicted or -1)] -- _c1_cache adds the tenants holding a region --, the error message, or None for a removal; fills;
+  // evictions).  _slot_cache: the key pager's (assignAll); _c1_cache: the c1 store's (assignByCount)
+  auto replayRegionCache = [](int regions, const std::vector<py::object> &ops, bool keySlots) {
+    RegionCache c(regions);
     py::list results;
     for (auto &op : ops) {
       if (py::isinstance<py::tuple>(op)) {   // ("remove", tenant)
@@ -182,38 +183,24 @@ PYBIND11_MODULE(_eva_b200, m) {
         results.append(py::none());
         continue;
       }
-      std::vector<SlotCache::Fill> fills;
+      std::vector<RegionCache::Fill> fills;
       try {
-        std::vector<int> s = c.assign(op.cast<std::vector<int>>(), fills);
+        const std::vector<int> batch = op.cast<std::vector<int>>();
+        std::vector<int> r = keySlots ? c.assignAll(batch, fills) : c.assignByCount(batch, fills);
         py::list fl;
-        for (auto &f : fills) fl.append(py::make_tuple(f.tenant, f.slot, f.evicted));
-        results.append(py::make_tuple(s, fl));
+        for (auto &f : fills) fl.append(py::make_tuple(f.tenant, f.region, f.evicted));
+        if (keySlots) results.append(py::make_tuple(r, fl));
+        else results.append(py::make_tuple(r, fl, c.holders()));
       } catch (const std::invalid_argument &e) {
         results.append(py::str(e.what()));
       }
     }
     return py::make_tuple(results, c.fills(), c.evictions());
-  }, py::arg("slots"), py::arg("batches"));
-  // test hook: the c1 cache's admission and eviction policy alone (host/slot_cache.hpp C1Cache), as _slot_cache.  Returns (per entry:
-  // (region of every instance or -1, [(tenant, region, evicted or -1)], the tenants holding a region), or None for a removal;
-  // fills; evictions)
-  m.def("_c1_cache", [](int regions, const std::vector<py::object> &ops) {
-    C1Cache c(regions);
-    py::list results;
-    for (auto &op : ops) {
-      if (py::isinstance<py::tuple>(op)) {   // ("remove", tenant)
-        c.drop(py::cast<int>(op.cast<py::tuple>()[1]));
-        results.append(py::none());
-        continue;
-      }
-      std::vector<C1Cache::Fill> fills;
-      std::vector<int> r = c.assign(op.cast<std::vector<int>>(), fills);
-      py::list fl;
-      for (auto &f : fills) fl.append(py::make_tuple(f.tenant, f.region, f.evicted));
-      results.append(py::make_tuple(r, fl, c.cached()));
-    }
-    return py::make_tuple(results, c.fills(), c.evictions());
-  }, py::arg("regions"), py::arg("batches"));
+  };
+  m.def("_slot_cache", [=](int slots, const std::vector<py::object> &ops) { return replayRegionCache(slots, ops, true); },
+        py::arg("slots"), py::arg("batches"));
+  m.def("_c1_cache", [=](int regions, const std::vector<py::object> &ops) { return replayRegionCache(regions, ops, false); },
+        py::arg("regions"), py::arg("batches"));
   // test hook: the planner alone (host/planner.hpp), without a device.  options: set_options' keywords; arena_limit 0 is no limit
   // here.  The scratch sizes are stand-ins derived from N and ell (the layout's invariants hold for any sizes)
   py::class_<ExecOptions> planOptions(m, "_PlanOptions");
@@ -665,7 +652,7 @@ PYBIND11_MODULE(_eva_b200, m) {
         d["device_slots"] = b.capacity();
         d["max_tenants"] = pg ? pg->maxTenants() : b.capacity();
         std::vector<int> resident;
-        if (pg) resident = pg->cache().resident();
+        if (pg) resident = pg->cache().holders();
         else for (int t = 0; t < b.capacity(); t++) if (b.occupied(t)) resident.push_back(t);
         d["resident"] = resident;
         d["host_key_bytes"] = pg ? pg->hostBytes() : 0;
@@ -679,7 +666,7 @@ PYBIND11_MODULE(_eva_b200, m) {
         const C1Store *c1 = s.shared()->c1.get();
         d["c1_cache"] = b.c1Regions();
         d["c1_cache_bytes"] = b.stride() * 8 * (std::size_t)b.c1Regions();
-        d["c1_cached"] = c1 ? c1->cache().cached() : std::vector<int>();
+        d["c1_cached"] = c1 ? c1->cache().holders() : std::vector<int>();
         d["c1_fills"] = c1 ? c1->cache().fills() : 0;
         d["c1_evictions"] = c1 ? c1->cache().evictions() : 0;
         const CipherStore *st = s.cipherStore();
