@@ -53,6 +53,10 @@ _SIGS = {
     "evab_expand_key_uniform": (ci, [vp, ci, vp, u64p, vp, vp]),
     "evab_expand_cipher_uniform": (ci, [vp, ci, vp, vp, vp, u64p, vp]),
     "evab_gather_ciphers": (ci, [vp, ci, vp, vp, u64p, vp]),
+    "evab_compact_work_bytes": (szt, [vp, ci, ci]),
+    "evab_compact_ciphers": (ci, [vp, ci, vp, vp, ci, ci, ci, vp, vp]),
+    "evab_compact_unpack": (ci, [vp, vp, ci, ci, vp, vp]),
+    "evab_compact_finish": (ci, [vp, vp, ci, ci, ci, vp, vp, vp]),
     "evab_rotate_modup_prepared": (ci, [vp, ci, vp, vp, vp, u64, vp, vp, vp, vp]),
     "evab_memset_zero": (ci, [vp, vp, szt, vp]),
     "evab_rotate_modup_scale_c0": (ci, [vp, ci, vp, vp, vp]),

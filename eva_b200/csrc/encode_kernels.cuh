@@ -11,6 +11,7 @@
 #pragma once
 #include "modarith.cuh"
 #include <math.h>
+#include <string.h>
 
 struct __align__(16) cplx { double re, im; };
 
@@ -145,6 +146,12 @@ EVAB_HD void enc_uniform_elem(const EncUniform &B, u32 e, u32 i, u32 j, long lon
 // order, explicit round-to-nearest, as the host decoder and the oracle (ora_decode): identical doubles.
 #define DEC_MAX_ELL 8
 #define DEC_WORDS (DEC_MAX_ELL + 1)
+// CRT constants of the first ell primes (multi-word, little-endian u64 words; ell + 1 words are used)
+struct CrtTables {
+  u64 Q[DEC_WORDS], halfQ[DEC_WORDS];        // Q = q_0 ... q_{ell-1}, (Q + 1) / 2
+  u64 punct[DEC_MAX_ELL][DEC_WORDS];         // Q / q_i
+  u64 ipunct[DEC_MAX_ELL];                   // (Q / q_i)^-1 mod q_i
+};
 struct DecArgs {
   const u64 *coef;              // [ell][N] coefficient-form residues
   cplx *work;                   // [N]
@@ -152,9 +159,7 @@ struct DecArgs {
   const cplx *roots;            // [N] zeta^bitrev(i)
   const u32 *slot_index;        // [N]
   const PrimeDev *primes;
-  u64 Q[DEC_WORDS], halfQ[DEC_WORDS];        // Q = q_0 ... q_{ell-1}, (Q + 1) / 2
-  u64 punct[DEC_MAX_ELL][DEC_WORDS];         // Q / q_i
-  u64 ipunct[DEC_MAX_ELL];                   // (Q / q_i)^-1 mod q_i
+  CrtTables T;
   double inv_scale;
   u32 N, ell;
 };
@@ -166,25 +171,30 @@ EVAB_HD void dec_sub(u64 *a, const u64 *b, int nw) {   // a -= b
   u64 borrow = 0;
   for (int i = 0; i < nw; i++) { const u64 t = a[i] - b[i], t2 = t - borrow; borrow = (a[i] < b[i]) | (t < borrow); a[i] = t2; }
 }
-// coefficient j -> work[j] = (centred CRT value / scale, 0)
-EVAB_HD void dec_compose(const DecArgs &A, u32 j) {
-  const int nw = (int)A.ell + 1;
-  u64 X[DEC_WORDS];
+// X (ell + 1 words) = the CRT composition in [0, Q) of the residues coef[i * stride], i < ell
+EVAB_HD void crt_compose(const CrtTables &T, const PrimeDev *primes, u32 ell, const u64 *coef, size_t stride, u64 *X) {
+  const int nw = (int)ell + 1;
   for (int w = 0; w < nw; w++) X[w] = 0;
-  for (u32 i = 0; i < A.ell; i++) {
-    const PrimeDev P = A.primes[i];
-    const u64 v = mulmod(A.coef[(size_t)i * A.N + j], A.ipunct[i], P.p, P.ratio_lo, P.ratio_hi);
+  for (u32 i = 0; i < ell; i++) {
+    const PrimeDev P = primes[i];
+    const u64 v = mulmod(coef[(size_t)i * stride], T.ipunct[i], P.p, P.ratio_lo, P.ratio_hi);
     u64 carry = 0;                                        // X += punct[i] * v
     for (int w = 0; w < nw; w++) {
-      const u64 lo = A.punct[i][w] * v, hi = mulhi64(A.punct[i][w], v);
+      const u64 lo = T.punct[i][w] * v, hi = mulhi64(T.punct[i][w], v);
       const u64 s = X[w] + lo, c1 = s < lo;
       const u64 s2 = s + carry, c2 = s2 < carry;
       X[w] = s2; carry = hi + c1 + c2;
     }
   }
-  while (dec_cmp(X, A.Q, nw) >= 0) dec_sub(X, A.Q, nw);
-  const bool neg = dec_cmp(X, A.halfQ, nw) >= 0;
-  if (neg) { u64 T[DEC_WORDS]; for (int w = 0; w < nw; w++) T[w] = A.Q[w]; dec_sub(T, X, nw); for (int w = 0; w < nw; w++) X[w] = T[w]; }
+  while (dec_cmp(X, T.Q, nw) >= 0) dec_sub(X, T.Q, nw);
+}
+// coefficient j -> work[j] = (centred CRT value / scale, 0)
+EVAB_HD void dec_compose(const DecArgs &A, u32 j) {
+  const int nw = (int)A.ell + 1;
+  u64 X[DEC_WORDS];
+  crt_compose(A.T, A.primes, A.ell, A.coef + j, A.N, X);
+  const bool neg = dec_cmp(X, A.T.halfQ, nw) >= 0;
+  if (neg) { u64 T[DEC_WORDS]; for (int w = 0; w < nw; w++) T[w] = A.T.Q[w]; dec_sub(T, X, nw); for (int w = 0; w < nw; w++) X[w] = T[w]; }
   double acc = 0.0, f = A.inv_scale;
   for (int w = 0; w < nw; w++) { if (X[w]) acc = D_ADD(acc, D_MUL((double)X[w], f)); f = D_MUL(f, 18446744073709551616.0); }
   cplx c; c.re = neg ? -acc : acc; c.im = 0.0;
@@ -202,3 +212,26 @@ EVAB_HD void dec_fft_bfly(const DecArgs &A, u32 m, u32 b) {
   w[j + t].re = D_SUB(ur, vr); w[j + t].im = D_SUB(ui, vi);
 }
 EVAB_HD void dec_gather(const DecArgs &A, u32 i) { A.out[i] = A.work[A.slot_index[i]].re; }
+
+// host: the CRT constants of primes[0 .. ell), 1 <= ell <= DEC_MAX_ELL
+inline void crt_tables(CrtTables &T, const u64 *primes, int ell) {
+  typedef unsigned __int128 u128;
+  const int nw = ell + 1;
+  memset(&T, 0, sizeof(T));
+  auto big_mul = [&](u64 *x, u64 m) { u64 carry = 0; for (int w = 0; w < nw; w++) { const u128 t = (u128)x[w] * m + carry; x[w] = (u64)t; carry = (u64)(t >> 64); } };
+  auto big_mod = [&](const u64 *x, u64 m) { u128 r = 0; for (int w = nw - 1; w >= 0; w--) r = ((r << 64) | x[w]) % m; return (u64)r; };
+  T.Q[0] = 1;
+  for (int i = 0; i < ell; i++) big_mul(T.Q, primes[i]);
+  for (int i = 0; i < ell; i++) {
+    T.punct[i][0] = 1;
+    for (int j = 0; j < ell; j++) if (j != i) big_mul(T.punct[i], primes[j]);
+    // inverse by Fermat: q_i prime
+    const u64 p = primes[i];
+    u64 base = big_mod(T.punct[i], p), e = p - 2, r = 1;
+    while (e) { if (e & 1) r = (u64)((u128)r * base % p); base = (u64)((u128)base * base % p); e >>= 1; }
+    T.ipunct[i] = r;
+  }
+  for (int w = 0; w < nw; w++) T.halfQ[w] = T.Q[w];
+  { u64 carry = 1; for (int w = 0; w < nw && carry; w++) { T.halfQ[w] += carry; carry = T.halfQ[w] == 0; } }
+  for (int w = 0; w < nw; w++) T.halfQ[w] = (T.halfQ[w] >> 1) | (w + 1 < nw ? T.halfQ[w + 1] << 63 : 0);
+}

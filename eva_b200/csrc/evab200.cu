@@ -6,6 +6,7 @@
 #include "host_tables.hpp"
 #include "ops_impl.hpp"
 #include "key_expand.cuh"
+#include "compact_kernels.cuh"
 #include <cuda_runtime.h>
 #include <algorithm>
 #include <atomic>
@@ -340,6 +341,21 @@ __global__ void __launch_bounds__(GW_THREADS) k_gather_words(const GatherArgs A)
     for (int u = 0; u < GW_UNROLL; u++)
       if (i + u * GW_THREADS < E.vecs) E.dst[i + u * GW_THREADS] = v[u];
   }
+}
+// ---- compact responses (evab_compact_ciphers): grid (tiles of output words, polynomial, entry of the launch); one thread per word
+static_assert(sizeof(CompactArgs) <= 4096, "the compaction's arguments must fit the classic 4 KB parameter space");
+__global__ void __launch_bounds__(CMP_THREADS) k_compact(const CompactArgs A) {
+  const u32 w = blockIdx.x * CMP_THREADS + threadIdx.x;
+  if (w < A.words) compact_word(A, blockIdx.z, blockIdx.y, w);
+}
+__global__ void __launch_bounds__(256) k_compact_unpack(const u64 *words, u32 b, u32 W, const PrimeDev *primes, u32 nres, u32 N, u64 *out) {
+  const u32 i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < N) compact_unpack_elem(words, b, W, primes, nres, N, out, i);
+}
+__global__ void __launch_bounds__(256) k_compact_finish(const CrtTables T, const PrimeDev *primes, u32 nres, u32 N, u32 b, const u64 *coef, u32 nout,
+                                                        u64 *out, long long *z) {
+  const u32 i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < N) compact_finish_elem(T, primes, nres, N, b, coef, nout, out, z, i);
 }
 __global__ void __launch_bounds__(256) k_hoist_indicator(u64 *out, const u32 *ctab, int N) {
   for (int j = blockIdx.x * blockDim.x + threadIdx.x; j < N; j += gridDim.x * blockDim.x) hoist_indicator_elem(out, ctab, N, blockIdx.y, j);
@@ -1202,5 +1218,82 @@ extern "C" int evab_gather_ciphers(evab_ctx *c, int n, const uint64_t *const *sr
     k_gather_words<<<dim3((unsigned)tiles, nb), GW_THREADS, 0, S(stream)>>>(A);
     CUDA_OK(cudaGetLastError());
   }
+  return 0;
+}
+
+// ---- compact responses
+extern "C" size_t evab_compact_work_bytes(const evab_ctx *c, int n, int ell) {
+  return n < 1 || ell < 1 ? 0 : (size_t)2 * n * ell * c->v.N * sizeof(u64);
+}
+extern "C" int evab_compact_ciphers(evab_ctx *c, int n, const uint64_t *const *src, uint64_t *const *dst, int ell, int shift, int bits, void *work,
+                                    void *stream) {
+  if (n < 0 || n > 32767) return fail("evab_compact_ciphers: n must be in [0, 32767]");
+  if (!src) return fail("evab_compact_ciphers: h_src is null");
+  if (!dst) return fail("evab_compact_ciphers: h_dst is null");
+  if (ell < 1 || ell > DEC_MAX_ELL || ell > c->v.k) return fail("evab_compact_ciphers: ell must be in [1, min(8, k)]");
+  if (bits < 1 || bits > 62) return fail("evab_compact_ciphers: bits must be in [1, 62]");
+  if (shift < bits) return fail("evab_compact_ciphers: shift must be >= bits");
+  if (!work || reinterpret_cast<uintptr_t>(work) % 16) return fail("evab_compact_ciphers: d_work is null or not 16-byte aligned");
+  for (int i = 0; i < n; i++) {
+    const std::string at = "[" + std::to_string(i) + "]";
+    if (!src[i] || reinterpret_cast<uintptr_t>(src[i]) % 16) return fail("evab_compact_ciphers: h_src" + at + " is null or not 16-byte aligned");
+    if (!dst[i] || reinterpret_cast<uintptr_t>(dst[i]) % 8) return fail("evab_compact_ciphers: h_dst" + at + " is null or not 8-byte aligned");
+  }
+  if (n == 0) return 0;
+  const size_t N = c->v.N, rows = (size_t)2 * ell * N;
+  // 1. the ciphertexts side by side in d_work
+  std::vector<uint64_t *> to(n);
+  std::vector<uint64_t> words(n, rows);
+  for (int i = 0; i < n; i++) to[i] = (uint64_t *)work + i * rows;
+  if (int rc = evab_gather_ciphers(c, n, src, to.data(), words.data(), stream)) return rc;
+  // 2. coefficient form: one transform of the 2 n ell rows (the call's own batch of one, whatever evab_set_batch says)
+  {
+    const BatchState saved = g_batch;
+    g_batch = BatchState();
+    int pidx[DEC_MAX_ELL];
+    for (int i = 0; i < ell; i++) pidx[i] = i;
+    int rc;
+    { BE_BEGIN rc = ntt_batch_impl(be, c->v, true, (u64 *)work, (size_t)2 * n * ell, pidx, ell); }
+    g_batch = saved;
+    if (rc) return rc;
+  }
+  // 3. CRT of x' = 2^(shift-bits) x mod Q, exact rounding, packing
+  CompactArgs A;
+  compact_args(A, c->primes.data(), ell, shift, bits, (u32)N);
+  A.primes = c->v.primes;
+  CUDA_OK(cudaSetDevice(c->device));
+  for (int i0 = 0; i0 < n; i0 += CMP_MAX_ENTRIES) {
+    const int nb = std::min(CMP_MAX_ENTRIES, n - i0);
+    A.src = (const u64 *)work + i0 * rows;
+    for (int b = 0; b < nb; b++) A.dst[b] = dst[i0 + b];
+    c->launches.fetch_add(1, std::memory_order_relaxed);
+    k_compact<<<dim3((A.words + CMP_THREADS - 1) / CMP_THREADS, 2, nb), CMP_THREADS, 0, S(stream)>>>(A);
+    CUDA_OK(cudaGetLastError());
+  }
+  return 0;
+}
+extern "C" int evab_compact_unpack(evab_ctx *c, const uint64_t *words, int bits, int nres, uint64_t *out, void *stream) {
+  if (!words || !out) return fail("evab_compact_unpack: d_words and d_out must not be null");
+  if (bits < 1 || bits > 62) return fail("evab_compact_unpack: bits must be in [1, 62]");
+  if (nres < 1 || nres > DEC_MAX_ELL || nres > c->v.k) return fail("evab_compact_unpack: nres must be in [1, min(8, k)]");
+  const u32 N = (u32)c->v.N;
+  CUDA_OK(cudaSetDevice(c->device));
+  c->launches.fetch_add(1, std::memory_order_relaxed);
+  k_compact_unpack<<<(N + 255) / 256, 256, 0, S(stream)>>>(words, (u32)bits, (u32)(((u64)N * bits + 63) / 64), c->v.primes, (u32)nres, N, out);
+  CUDA_OK(cudaGetLastError());
+  return 0;
+}
+extern "C" int evab_compact_finish(evab_ctx *c, const uint64_t *coef, int nres, int bits, int nout, uint64_t *out, int64_t *z, void *stream) {
+  if (!coef || !out) return fail("evab_compact_finish: d_coef and d_out must not be null");
+  if (bits < 1 || bits > 62) return fail("evab_compact_finish: bits must be in [1, 62]");
+  if (nres < 1 || nres > DEC_MAX_ELL || nres > c->v.k) return fail("evab_compact_finish: nres must be in [1, min(8, k)]");
+  if (nout < 1 || nout > DEC_MAX_ELL || nout > c->v.k) return fail("evab_compact_finish: nout must be in [1, min(8, k)]");
+  CrtTables T;
+  crt_tables(T, c->primes.data(), nres);
+  const u32 N = (u32)c->v.N;
+  CUDA_OK(cudaSetDevice(c->device));
+  c->launches.fetch_add(1, std::memory_order_relaxed);
+  k_compact_finish<<<(N + 255) / 256, 256, 0, S(stream)>>>(T, c->v.primes, (u32)nres, N, (u32)bits, coef, (u32)nout, out, (long long *)z);
+  CUDA_OK(cudaGetLastError());
   return 0;
 }

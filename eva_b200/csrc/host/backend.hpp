@@ -59,7 +59,36 @@ struct HostPlain { HostBuf data; int ell = 0; double scale = 0; };
 struct HostSeededCipher { HostBuf c0; int ell = 0; double scale = 0; KeySeed seed{}; };
 // a reference to a ciphertext held in a B200Server's store (CipherStore): the handle alone; level, scale and words are the entry's
 struct StoredCipher { std::uint64_t handle = 0; };
-using SchemeValue = std::variant<HostCipher, HostPlain, std::shared_ptr<ConstantValue>, HostSeededCipher, StoredCipher>;
+// a compact response (B200Public compact_outputs): an output ciphertext switched to the modulus 2^bits and bit-packed,
+// words [2][W], W = ceil(N bits / 64) (compact_kernels.cuh); scale is the compact scale.  Decrypted by B200Secret, never a program input
+struct HostCompactCipher { HostBuf words; int bits = 0; double scale = 0; };
+using SchemeValue = std::variant<HostCipher, HostPlain, std::shared_ptr<ConstantValue>, HostSeededCipher, StoredCipher, HostCompactCipher>;
+
+// Compact responses: the modulus 2^bits an output ciphertext at `ell` residues, scale `scale` and declared range `range` (bits) is
+// switched to for `precision` bits after the binary point, with margin m = log2 N + 1 for the rounding noise r0 + r1 s.
+//   shift = ceil(log2(Q / scale)) + precision + m,  bits = min(shift, range + precision + m + 2),  compact scale = scale 2^shift / Q
+// (log2 Q is the sum of log2 q_i).  The whole policy: the output stays a full ciphertext when it is not a ciphertext, has size 3,
+// declares no range (no width can be derived), has more than kCompactMaxEll residues (the CRT limit of the compaction kernel),
+// bits >= floor(log2 Q) (nothing would shrink) or bits > 62.  Decided on the host before anything of a batch is enqueued
+constexpr int kCompactMaxEll = 8;   // evab_compact_ciphers / evab_compact_finish / evab_decode residue limit
+struct CompactShape { bool compact = false; int shift = 0, bits = 0; double scale = 0; };
+inline CompactShape compactShape(const std::vector<u64> &primes, bool cipher, int size, int ell, double scale, std::optional<std::uint32_t> range,
+                                 int precision, u64 N) {
+  CompactShape c;
+  if (!cipher || size != 2 || !range || ell < 1 || ell > (int)primes.size()) return c;
+  double log2Q = 0;
+  for (int i = 0; i < ell; i++) log2Q += std::log2((double)primes[i]);
+  const int m = (int)std::log2((double)N) + 1;
+  c.shift = (int)std::ceil(log2Q - std::log2(scale)) + precision + m;
+  c.bits = std::min(c.shift, (int)*range + precision + m + 2);
+  c.scale = std::pow(2.0, std::log2(scale) + c.shift - log2Q);
+  c.compact = c.bits < (int)std::floor(log2Q) && c.bits <= 62 && ell <= kCompactMaxEll;
+  return c;
+}
+// the one refusal of a compact value where a ciphertext is expected
+inline std::invalid_argument compactRefused(const std::string &what) {
+  return std::invalid_argument(what + " is a compact response (compact_outputs): it can only be decrypted, not sent to a program or stored");
+}
 
 class B200Valuation {
 public:
@@ -279,6 +308,7 @@ public:
         if (sc->ell < 1 || sc->ell > k - 1 || sc->c0.size() != (std::size_t)sc->ell * N)
           throw std::invalid_argument(what + ": seeded ciphertext does not match the server's parameters (level / degree)");
       } else {
+        if (std::holds_alternative<HostCompactCipher>(kv.second)) throw compactRefused(what);
         const char *kind = std::holds_alternative<HostPlain>(kv.second) ? "a plaintext" : std::holds_alternative<StoredCipher>(kv.second) ? "a stored reference" : "a raw vector";
         throw std::invalid_argument(what + " is " + kind + ": only ciphertexts can be stored");
       }
@@ -424,6 +454,7 @@ inline B200Valuation encodeInputs(Shared &s, const Valuation &inputs, const CKKS
 struct PlanHolder {
   std::shared_ptr<Shared> keepAlive;  // the plan references the context's encoder and keys
   std::unique_ptr<Executor> exec;
+  DBuf compactScratch;                // compact_outputs: the replica's compaction work area and packed words, made on first use
   std::uint64_t termCount = 0;
   ExecOptions opt;
 };
@@ -436,6 +467,7 @@ struct PendingBatch {
   std::vector<void *> streams;
   std::vector<std::shared_ptr<PlanHolder>> plans;   // the plans it runs on stay alive until it is collected (set_options may replace them meanwhile)
   std::vector<int> tenants;                         // key-bank tenant of every instance (B200Server), empty with a single key set
+  int compact = 0;                                  // compact_outputs precision at submit (0: full outputs); collect's redo keeps it
   int slot = 0;
   bool collected = false;
   std::shared_ptr<Shared> keep;
@@ -515,6 +547,8 @@ public:
         } else if (auto *r = std::get_if<StoredCipher>(&in.second)) {
           if (!s_->store || !s_->store->find(r->handle)) throw std::logic_error("input " + in.first + ": stored reference staged without checkStored");
           gatherSrc.push_back(s_->store->words(r->handle)); gatherDst.push_back(ex.valuePtr(term, b)); gatherWords.push_back((u64)2 * vi.ell * N);
+        } else if (std::holds_alternative<HostCompactCipher>(in.second)) {
+          throw compactRefused("input " + in.first);
         } else if (auto *p = std::get_if<HostPlain>(&in.second)) {
           if (vi.kind != Kind::Plain || p->ell != vi.ell || p->data.size() != (std::size_t)vi.ell * N)
             throw std::runtime_error("input " + in.first + ": plaintext does not match the program signature");
@@ -570,8 +604,11 @@ public:
   // call's ciphertext.  The reference builds a fresh executor per call and fails on the missing value
   // (seal_executor.h:264); so does this.
   static void requireAllInputs(Program &program, const B200Valuation &inputs) {
-    for (auto &in : program.getInputs())
-      if (inputs.values.find(in.first) == inputs.values.end()) throw std::runtime_error("Missing input value: " + in.first);
+    for (auto &in : program.getInputs()) {
+      auto it = inputs.values.find(in.first);
+      if (it == inputs.values.end()) throw std::runtime_error("Missing input value: " + in.first);
+      if (std::holds_alternative<HostCompactCipher>(it->second)) throw compactRefused("input " + in.first);
+    }
   }
   // SEALPublic::execute -- reference eva/seal/seal.cpp:104-122.  Host buffers in,
   // host buffers out: H2D of the inputs, the DAG on the GPU, D2H of the outputs.
@@ -590,15 +627,17 @@ public:
   // B valuations are split into chunks of options.fuse instances; every chunk has its own plan
   // replica (arena + captured graph) and all replicas are in flight at once: H2D, graph and D2H of
   // different chunks overlap, and the SMs are filled by concurrency rather than by launch width.
-  std::vector<B200Valuation> executeMany(Program &program, const std::vector<const B200Valuation *> &inputs) {
-    auto p = submitMany(program, inputs, 0);
+  std::vector<B200Valuation> executeMany(Program &program, const std::vector<const B200Valuation *> &inputs, int compact = -1) {
+    auto p = submitMany(program, inputs, 0, {}, compact);
     return collect(*p);
   }
   // Pipelined form of executeMany: submitMany enqueues a batch (H2D of its inputs, the plan replays, D2H of its outputs) and returns;
   // collect waits for it and hands out the results.  Batches submitted with different `slot` numbers (0..7) use disjoint plan
   // replicas, so the head of one overlaps the tail of the other (each batch alone ramps up replica by replica and drains the same way).
   // tenants: with a key bank (B200Server), the tenant whose keys instance b runs with; otherwise empty
-  std::shared_ptr<PendingBatch> submitMany(Program &program, const std::vector<const B200Valuation *> &inputs, int slot = 0, std::vector<int> tenants = {}) {
+  // compact: the compact_outputs precision of this batch (-1: the context's option)
+  std::shared_ptr<PendingBatch> submitMany(Program &program, const std::vector<const B200Valuation *> &inputs, int slot = 0, std::vector<int> tenants = {},
+                                           int compact = -1) {
     if (inputs.empty()) throw std::invalid_argument("execute needs at least one valuation");
     if (slot < 0 || slot > 7) throw std::invalid_argument("slot out of range (0..7)");
     if (s_->bank ? tenants.size() != inputs.size() : !tenants.empty()) throw std::invalid_argument("one tenant per valuation on a key bank, none otherwise");
@@ -610,6 +649,7 @@ public:
     if (auto prev = inFlight_[slot].lock(); prev && !prev->collected) throw std::runtime_error("slot in use: collect the batch submitted before");
     auto p = std::make_shared<PendingBatch>();
     p->program = &program; p->inputs = inputs; p->slot = slot; p->keep = s_; p->tenants = std::move(tenants);
+    p->compact = compact < 0 ? compactOutputs : compact;
     enqueueLocked(*p);
     inFlight_[slot] = p;
     return p;
@@ -685,6 +725,7 @@ public:
       s_->beforeRun(st, res, b0, nb);
       ex.run(st);
       s_->afterRun(st, res, b0, nb);
+      if (p.compact) compactOutputsOf(*holder, program, p.compact, outs.data() + b0, nb, st);
       auto t3 = now();
       tPlan += std::chrono::duration<double>(t1 - t0).count(); tStage += std::chrono::duration<double>(t2 - t1).count();
       tRun += std::chrono::duration<double>(t3 - t2).count();
@@ -692,6 +733,7 @@ public:
         for (auto &o : program.getOutputs()) {
           const ValueInfo &vi = ex.info(o.second);
           B200Valuation &out = outs[b0 + b];
+          if (out.values.count(o.first)) continue;   // compacted
           if (vi.kind == Kind::Cipher) {
             HostCipher h; h.size = vi.size; h.ell = vi.ell; h.scale = vi.scale; h.data.resize((std::size_t)vi.size * vi.ell * N);
             s_->dev->download(h.data.data(), ex.valuePtr(o.second, b), h.data.size() * 8, st);
@@ -709,6 +751,38 @@ public:
       std::fprintf(stderr, "[evab] enqueue B=%d F=%d slot=%d: plan %.3f stage %.3f run %.3f enqueue-total %.3f ms\n", B, F, p.slot, tPlan * 1e3, tStage * 1e3, tRun * 1e3,
                    std::chrono::duration<double>(now() - t00).count() * 1e3);
   }
+  // compact responses of a chunk of nb instances just run on `st` by the replica `h`: every output that compactShape compacts at
+  // precision p is switched and packed on the device by one evab_compact_ciphers call over the chunk, then only its packed words are
+  // downloaded into outs[b][name].  The scratch is the replica's own (no allocation on the steady path; nothing while the option is
+  // off): its chunks run in order on `st`, and each output's downloads are enqueued before the next compaction rewrites the words
+  void compactOutputsOf(PlanHolder &h, Program &program, int p, B200Valuation *outs, int nb, void *st) {
+    const u64 N = s_->dev->N();
+    evab_ctx *ctx = s_->dev->ctx();
+    Executor &ex = *h.exec;
+    for (auto &o : program.getOutputs()) {
+      const ValueInfo &vi = ex.info(o.second);
+      const CompactShape cs = compactShape(s_->dev->primes(), vi.kind == Kind::Cipher, vi.size, vi.ell, vi.scale, o.second->range, p, N);
+      if (!cs.compact) continue;
+      const std::size_t W = (N * cs.bits + 63) / 64;
+      const std::size_t workWords = evab_compact_work_bytes(ctx, nb, vi.ell) / 8, need = workWords + (std::size_t)nb * 2 * W;
+      if (h.compactScratch.words() < need) {
+        s_->dev->sync(st);                        // the replica's earlier chunks may still use the old area
+        h.compactScratch = DBuf();
+        h.compactScratch = DBuf(s_->dev, need);
+        s_->dev->sync();                          // allocated before `st` uses it
+      }
+      u64 *work = h.compactScratch.get(), *dst = work + workWords;
+      std::vector<const u64 *> src(nb);
+      std::vector<u64 *> to(nb);
+      for (int b = 0; b < nb; b++) { src[b] = ex.valuePtr(o.second, b); to[b] = dst + (std::size_t)b * 2 * W; }
+      check(evab_compact_ciphers(ctx, nb, src.data(), to.data(), vi.ell, cs.shift, cs.bits, work, st));
+      for (int b = 0; b < nb; b++) {
+        HostCompactCipher hc; hc.bits = cs.bits; hc.scale = cs.scale; hc.words.resize(2 * W);
+        s_->dev->download(hc.words.data(), to[b], 2 * W * 8, st);
+        outs[b][o.first] = std::move(hc);
+      }
+    }
+  }
   // with execMutex held: does a submitted, not yet collected batch run an instance with this tenant's keys?
   bool tenantInFlightLocked(int t) const {
     for (auto &w : inFlight_)
@@ -717,6 +791,7 @@ public:
   }
   std::shared_ptr<Shared> shared() const { return s_; }
   ExecOptions options;
+  int compactOutputs = 0;         // compact responses: bits of precision after the binary point (0: off); shapes no plan
   std::uint64_t plansBuilt = 0;   // executors constructed by this context (plan build + arena + graph capture each)
 
 private:
@@ -924,12 +999,51 @@ public:
       } else if (auto *r = std::get_if<StoredCipher>(&e.second)) {
         throw std::invalid_argument("value " + e.first + " is a reference to a stored ciphertext (handle " + std::to_string(r->handle) +
                                     "): only a server's requests can name one");
+      } else if (auto *cc = std::get_if<HostCompactCipher>(&e.second)) {
+        out[e.first] = decryptCompact(*cc, e.first, nullptr);
       } else {
         std::get<std::shared_ptr<ConstantValue>>(e.second)->expandTo(out[e.first], sig.vecSize);
       }
       out.at(e.first).resize(sig.vecSize);
     }
     return out;
+  }
+  // a compact response: z = (y0 + y1 s) mod 2^bits, centred, decoded at the compact scale.  y1 s is exact in RNS over the fewest
+  // primes whose bit lengths sum to at least bits + 2 + log2 N (their product exceeds 2 (N+1) 2^bits); z is decoded over the fewest
+  // whose bit lengths sum to at least bits + 1.  z (if not null) receives the N centred integers
+  std::vector<double> decryptCompact(const HostCompactCipher &c, const std::string &name, std::vector<std::int64_t> *z) {
+    if (!s_->keys.sk) throw std::runtime_error("this context has no secret key");
+    const u64 N = s_->dev->N();
+    const auto &primes = s_->dev->primes();
+    const int k = s_->dev->k();
+    if (c.bits < 1 || c.bits > 62) throw std::invalid_argument("value " + name + ": compact ciphertext bits must be in [1, 62]");
+    const std::size_t W = (N * c.bits + 63) / 64;
+    if (c.words.size() != 2 * W) throw std::invalid_argument("value " + name + ": compact ciphertext does not match the parameters (2 x W words)");
+    auto fewest = [&](int need) {
+      int have = 0;
+      for (int i = 0; i < k && i < kCompactMaxEll; i++) { have += 63 - __builtin_clzll(primes[i]); if (have >= need) return i + 1; }
+      throw std::runtime_error("value " + name + ": the modulus chain is too short to decrypt a " + std::to_string(c.bits) + "-bit compact ciphertext");
+    };
+    const int logN = 63 - __builtin_clzll(N);
+    const int L = fewest(c.bits + 2 + logN), L2 = fewest(c.bits + 1);
+    evab_ctx *ctx = s_->dev->ctx();
+    std::vector<int> idx(std::max(L, L2));
+    for (std::size_t i = 0; i < idx.size(); i++) idx[i] = (int)i;
+    DBuf w(s_->dev, 2 * W), y(s_->dev, 2 * (std::size_t)L * N), t(s_->dev, (std::size_t)L * N), pt(s_->dev, (std::size_t)L2 * N), zd(s_->dev, N);
+    s_->dev->upload(w.get(), c.words.data(), 2 * W * 8);
+    check(evab_compact_unpack(ctx, w.get(), c.bits, L, y.get(), nullptr));
+    check(evab_ntt_fwd(ctx, y.get(), 2 * (std::size_t)L, idx.data(), L, nullptr));
+    check(evab_mul_plain(ctx, L, t.get(), y.get() + (std::size_t)L * N, 1, s_->keys.sk.get(), nullptr));
+    check(evab_add(ctx, L, t.get(), t.get(), 1, y.get(), 1, nullptr));
+    check(evab_ntt_inv(ctx, t.get(), (std::size_t)L, idx.data(), L, nullptr));
+    check(evab_compact_finish(ctx, t.get(), L, c.bits, L2, pt.get(), reinterpret_cast<std::int64_t *>(zd.get()), nullptr));
+    if (z) {
+      z->resize(N);
+      s_->dev->download(z->data(), zd.get(), N * 8);
+    }
+    check(evab_ntt_fwd(ctx, pt.get(), (std::size_t)L2, idx.data(), L2, nullptr));
+    s_->dev->sync();
+    return s_->client->encoder().decode(pt.get(), L2, c.scale);
   }
   std::shared_ptr<Shared> shared() const { return s_; }
 private:

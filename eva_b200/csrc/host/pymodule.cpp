@@ -56,9 +56,16 @@ static u64arr encryptSeededPoly(const std::shared_ptr<Shared> &s, const u64arr &
 static ExecOptions &optionsOf(B200Public &p) { return p.options; }
 static ExecOptions &optionsOf(B200Server &s) { return s.pub().options; }
 static ExecOptions &optionsOf(ExecOptions &o) { return o; }
+// compact_outputs belongs to the context, not to its plans (the planner hook has none)
+static int *compactOf(B200Public &p) { return &p.compactOutputs; }
+static int *compactOf(B200Server &s) { return &s.pub().compactOutputs; }
+static int *compactOf(ExecOptions &) { return nullptr; }
 template <class Self>
 static void setOptions(Self &self, int streams, bool graph, bool cache, bool dedup, int fuse, bool fuseSums, bool hoist, bool uniformEncode, bool dedupTerms,
-                       bool hoistModUp, bool approxHoist, int rotationChunk, std::size_t arenaLimit, bool rotationSums) {
+                       bool hoistModUp, bool approxHoist, int rotationChunk, std::size_t arenaLimit, bool rotationSums, int compactOutputs) {
+  if (compactOutputs < 0 || compactOutputs > 52)
+    throw py::value_error("compact_outputs (" + std::to_string(compactOutputs) + ") must be 0 (off) or the precision in bits, 1 .. 52");
+  if (int *c = compactOf(self)) *c = compactOutputs;
   ExecOptions &o = optionsOf(self);
   o.numStreams = streams; o.useGraph = graph; o.cacheConstants = cache; o.dedupConstants = dedup;
   o.fuse = fuse; o.fuseSums = fuseSums; o.hoistRotations = hoist; o.uniformEncode = uniformEncode;
@@ -70,10 +77,12 @@ static void defSetOptions(Class &cls) {
   cls.def("set_options", &setOptions<typename Class::type>,
           py::arg("num_streams") = 8, py::arg("use_graph") = true, py::arg("cache_constants") = true, py::arg("dedup_constants") = true,
           py::arg("fuse") = 1, py::arg("fuse_sums") = true, py::arg("hoist_rotations") = true, py::arg("uniform_encode") = true, py::arg("dedup_terms") = true, py::arg("hoist_mod_up") = true, py::arg("approx_hoist") = false, py::arg("rotation_chunk") = 16,
-          py::arg("arena_limit") = 0, py::arg("rotation_sums") = true,
+          py::arg("arena_limit") = 0, py::arg("rotation_sums") = true, py::arg("compact_outputs") = 0,
           "arena_limit: bytes one plan's arena may take (0: the free device memory when the plan is built).  A plan whose one-offset-per-value "
           "layout does not fit reuses the storage of dead values; if even that exceeds the limit, building the plan raises RuntimeError.  "
-          "rotation_sums: sums of rotations of one ciphertext weighted by scalar constants run as one bit-exact evab_rotate_wsum call (approx_hoist takes precedence)");
+          "rotation_sums: sums of rotations of one ciphertext weighted by scalar constants run as one bit-exact evab_rotate_wsum call (approx_hoist takes precedence).  "
+          "compact_outputs: 0 (off) or p in 1 .. 52: every size-2 output ciphertext is switched on the GPU to the modulus 2^b its declared range "
+          "and p bits after the binary point need, and returned bit-packed (B200Valuation kind \"compact_cipher\"); builds no plan");
 }
 
 // execute_batch_async handle: the batch plus the Python objects it reads from.  Destroyed with the GIL held (the batch first:
@@ -243,6 +252,15 @@ PYBIND11_MODULE(_eva_b200, m) {
   }, py::arg("program"), py::arg("N"), py::arg("k"), py::arg("options") = py::dict(), py::arg("batch") = 1, py::arg("galois_elements") = py::none());
   // test hook: the steps that get a Galois key under generate_keys / B200Server(rotation_keys=...)
   m.def("_rotation_key_steps", &rotationKeySteps, py::arg("params"), py::arg("rotation_keys"));
+  // test hook: the width rule of compact responses (backend.hpp compactShape) -> (compact, shift, bits, compact scale)
+  // range None: the output declares none; cipher / size: the output's kind and polynomial count
+  m.def("_compact_shape", [](const std::vector<u64> &primes, int ell, double scale, std::optional<std::uint32_t> range, int precision, u64 N, int size,
+                             bool cipher) {
+    if (ell < 1 || ell > (int)primes.size()) throw std::invalid_argument("ell out of range");
+    const CompactShape c = compactShape(primes, cipher, size, ell, scale, range, precision, N);
+    return py::make_tuple(c.compact, c.shift, c.bits, c.scale);
+  }, py::arg("primes"), py::arg("ell"), py::arg("scale"), py::arg("range"), py::arg("precision"), py::arg("N"), py::arg("size") = 2,
+     py::arg("cipher") = true);
   m.def("set_num_threads", [](int) {}, py::arg("num_threads"),
         "Kept for API compatibility: the DAG is scheduled on CUDA streams, not CPU threads.");
   py::class_<int>(m, "_GaloisGuard").def(py::init());
@@ -318,18 +336,47 @@ PYBIND11_MODULE(_eva_b200, m) {
           return py::make_tuple("seeded_cipher", a, sc->scale);
         }
         if (auto *r = std::get_if<StoredCipher>(&sv)) return py::make_tuple("stored", r->handle, py::none());
+        if (auto *cc = std::get_if<HostCompactCipher>(&sv)) {
+          const std::size_t W = cc->words.size() / 2;
+          u64arr a({(std::size_t)2, W});
+          std::memcpy(a.mutable_data(), cc->words.data(), cc->words.size() * 8);
+          return py::make_tuple("compact_cipher", a, cc->scale);
+        }
         return py::make_tuple("raw", std::get<std::shared_ptr<ConstantValue>>(sv)->values(), 0.0);
       })
       .def("set_stored", [](B200Valuation &v, const std::string &name, std::uint64_t handle) { v[name] = StoredCipher{handle}; },
            py::arg("name"), py::arg("handle"),
            "a reference to a ciphertext in a B200Server's store (B200Server.store returns the handles): the server stages the stored "
-           "entry where this valuation would carry the ciphertext");
+           "entry where this valuation would carry the ciphertext")
+      .def("compact_bits", [](const B200Valuation &v, const std::string &name) {
+        auto *cc = std::get_if<HostCompactCipher>(&v.at(name));
+        if (!cc) throw std::invalid_argument("value " + name + " is not a compact ciphertext");
+        return cc->bits;
+      }, py::arg("name"), "the modulus bits b of a compact response")
+      .def("set_compact_cipher", [](B200Valuation &v, const std::string &name, const u64arr &words, int bits, double scale) {
+        if (bits < 1 || bits > 62) throw std::invalid_argument("compact ciphertext " + name + ": bits (" + std::to_string(bits) + ") must be in [1, 62]");
+        if (words.ndim() != 2 || words.shape(0) != 2 || words.shape(1) < 1)
+          throw std::invalid_argument("compact ciphertext " + name + ": words must be [2][W]");
+        const std::size_t W = words.shape(1);
+        // W = ceil(N bits / 64) for a power of two N: the smallest N it holds must be the largest too
+        std::size_t N = 1;
+        while ((N * 2 * bits + 63) / 64 <= W && N < ((std::size_t)1 << 20)) N *= 2;
+        if ((N * bits + 63) / 64 != W) throw std::invalid_argument("compact ciphertext " + name + ": " + std::to_string(W) + " words per polynomial is not ceil(N bits / 64) for any N");
+        HostCompactCipher h; h.words = toHostBuf(words); h.bits = bits; h.scale = scale;
+        v[name] = std::move(h);
+      }, py::arg("name"), py::arg("words"), py::arg("bits"), py::arg("scale"),
+         "a compact response: words [2][ceil(N bits / 64)] (two bit-packed polynomials of N bits-bit fields), the compact scale");
 
   py::class_<PyPending, std::shared_ptr<PyPending>>(mb, "PendingBatch", "a submitted, not yet collected execute_batch");
   py::class_<B200Public> pub(mb, "B200Public", "The public part of the context: encryption and execution on the GPU");
   pub.def("encrypt", &B200Public::encrypt, py::arg("inputs"), py::arg("signature"))
       .def("execute", &B200Public::execute, py::arg("program"), py::arg("inputs"), py::call_guard<py::gil_scoped_release>())
       // the list is converted to pointers to the caller's valuations: no copy of the host ciphertexts
+      .def("execute_full", [](B200Public &p, Program &prog, const B200Valuation &in) {
+             std::vector<const B200Valuation *> v{&in};
+             return std::move(p.executeMany(prog, v, 0)[0]);
+           }, py::arg("program"), py::arg("inputs"), py::call_guard<py::gil_scoped_release>(),
+           "execute() with full output ciphertexts whatever compact_outputs says (the sharded modes run their parts with it)")
       .def("execute_batch", [](B200Public &p, Program &prog, const std::vector<const B200Valuation *> &in) { return p.executeMany(prog, in); },
            py::arg("program"), py::arg("inputs"), py::call_guard<py::gil_scoped_release>(),
            "Execute one compiled program on a list of valuations with batched kernels; returns a list of valuations")
@@ -497,6 +544,16 @@ PYBIND11_MODULE(_eva_b200, m) {
         s->dev->sync();
         return a;
       }, py::arg("ciphertext"))
+      // test hook: the centred integers z = (y0 + y1 s) mod 2^bits of a compact ciphertext [2][W], before decoding
+      .def("decrypt_compact_poly", [](B200Secret &x, const u64arr &words, int bits) {
+        if (words.ndim() != 2 || words.shape(0) != 2) throw std::invalid_argument("compact ciphertext words must be [2][W]");
+        HostCompactCipher h; h.words = toHostBuf(words); h.bits = bits; h.scale = 1.0;
+        std::vector<std::int64_t> z;
+        x.decryptCompact(h, "compact ciphertext", &z);
+        py::array_t<std::int64_t> a(z.size());
+        std::memcpy(a.mutable_data(), z.data(), z.size() * 8);
+        return a;
+      }, py::arg("words"), py::arg("bits"))
       .def("decode", [](B200Secret &x, const u64arr &pt, double scale) {
         auto s = x.shared();
         DBuf d(s->dev, pt.size());

@@ -614,26 +614,9 @@ inline size_t decode_tmp_elems(const CtxView &c, int ell) { return (size_t)ell *
 template <class BE>
 int decode_impl(BE &be, const CtxView &c, int ell, const u64 *primes_host, const u64 *pt, double scale, double *out, u64 *tmp, cplx *work) {
   if (ell < 1 || ell > c.k || ell > DEC_MAX_ELL) return be.error("decode: ell out of range (1..8)");
-  typedef unsigned __int128 u128;
-  const int nw = ell + 1;
   DecArgs A;
   memset(&A, 0, sizeof(A));
-  auto big_mul = [&](u64 *x, u64 m) { u64 carry = 0; for (int w = 0; w < nw; w++) { const u128 t = (u128)x[w] * m + carry; x[w] = (u64)t; carry = (u64)(t >> 64); } };
-  auto big_mod = [&](const u64 *x, u64 m) { u128 r = 0; for (int w = nw - 1; w >= 0; w--) r = ((r << 64) | x[w]) % m; return (u64)r; };
-  A.Q[0] = 1;
-  for (int i = 0; i < ell; i++) big_mul(A.Q, primes_host[i]);
-  for (int i = 0; i < ell; i++) {
-    A.punct[i][0] = 1;
-    for (int j = 0; j < ell; j++) if (j != i) big_mul(A.punct[i], primes_host[j]);
-    // inverse by Fermat: q_i prime
-    const u64 p = primes_host[i];
-    u64 base = big_mod(A.punct[i], p), e = p - 2, r = 1;
-    while (e) { if (e & 1) r = (u64)((u128)r * base % p); base = (u64)((u128)base * base % p); e >>= 1; }
-    A.ipunct[i] = r;
-  }
-  for (int w = 0; w < nw; w++) A.halfQ[w] = A.Q[w];
-  { u64 carry = 1; for (int w = 0; w < nw && carry; w++) { A.halfQ[w] += carry; carry = A.halfQ[w] == 0; } }
-  for (int w = 0; w < nw; w++) A.halfQ[w] = (A.halfQ[w] >> 1) | (w + 1 < nw ? A.halfQ[w + 1] << 63 : 0);
+  crt_tables(A.T, primes_host, ell);
   // coefficient form
   if (int rc = copy_impl(be, c, ell, ell, tmp, pt, 1)) return rc;
   int pidx[32];

@@ -569,6 +569,8 @@ def _subset(inputs, names):
                 out.set_cipher(name, arr, scale)
             elif kind == "seeded_cipher":      # carried compressed: the instance that stages it expands c1
                 out.set_seeded_cipher(name, arr, inputs.get_seed(name), scale)
+            elif kind == "compact_cipher":     # a response, never an input
+                raise ValueError("input %s is a compact response (compact_outputs): it can only be decrypted" % name)
             elif kind == "stored":             # the entry lives in one server's store; a B200Public has none
                 raise ValueError("input %s is a reference to a stored ciphertext (handle %d): the sharded modes run on B200Public "
                                  "contexts, which have no store; send the ciphertext inline" % (name, arr))
@@ -643,7 +645,7 @@ class AutoShardedRunner:
             return min(ts[1:])
         t_sh = torch.tensor([best(lambda: self.runner.run(inputs))], dtype=torch.float64, device="cuda")
         dist.all_reduce(t_sh, op=dist.ReduceOp.MAX)
-        t_single = best(lambda: self.pub.execute(self.prog, inputs) if self.rank == 0 else None)
+        t_single = best(lambda: self.pub.execute_full(self.prog, inputs) if self.rank == 0 else None)
         verdict = torch.tensor([1 if (self.rank == 0 and t_sh.item() < 0.97 * t_single) else 0], dtype=torch.int64, device="cuda")
         dist.broadcast(verdict, src=0)
         self.use_sharded = bool(verdict.item())
@@ -653,4 +655,4 @@ class AutoShardedRunner:
     def run(self, inputs):
         if self.use_sharded:
             return self.runner.run(inputs)
-        return self.pub.execute(self.prog, inputs) if self.rank == 0 else None
+        return self.pub.execute_full(self.prog, inputs) if self.rank == 0 else None

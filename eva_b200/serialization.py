@@ -148,6 +148,9 @@ COMPRESSED_CIPHERTEXT = 18
 # payload kind of a reference to a ciphertext kept in a B200Server's store, under the CIPHERTEXT object: the store's handle as a
 # one-element u64 array
 STORED_CIPHERTEXT = 19
+# payload kind of a compact response (compact_outputs), under the CIPHERTEXT object: the packed words [2][W] with the compact scale,
+# and in the header's extra words the modulus bits b
+COMPACT_CIPHERTEXT = 20
 
 
 # ------------------------------------------------------------------ Program / parameters / signature
@@ -384,6 +387,9 @@ def valuation_to_msg(val):
         elif kind == "stored":
             o = msg.values[name]
             o.seal_type, o.data = CIPHERTEXT, _pack(STORED_CIPHERTEXT, np.array([arr], dtype=np.uint64))
+        elif kind == "compact_cipher":
+            o = msg.values[name]
+            o.seal_type, o.data = CIPHERTEXT, _pack(COMPACT_CIPHERTEXT, arr, scale, extra=(val.compact_bits(name),))
         elif kind == "plain":
             o = msg.values[name]
             o.seal_type, o.data = PLAINTEXT, _pack(PLAINTEXT, arr, scale)
@@ -403,6 +409,11 @@ def valuation_from_msg(msg):
             if len(words) != 4:
                 raise RuntimeError("compressed ciphertext %s: the seed must be 32 bytes" % name)
             val.set_seeded_cipher(name, arr, _seed_bytes(words), scale)
+        elif o.seal_type == CIPHERTEXT and _kind(o.data) == COMPACT_CIPHERTEXT:
+            arr, scale, words = _unpack(o.data, COMPACT_CIPHERTEXT)
+            if len(words) != 1:
+                raise RuntimeError("compact ciphertext %s: the header must carry the modulus bits" % name)
+            val.set_compact_cipher(name, arr, int(words[0]), scale)
         elif o.seal_type == CIPHERTEXT and _kind(o.data) == STORED_CIPHERTEXT:
             arr, _, words = _unpack(o.data, STORED_CIPHERTEXT)
             if arr.shape != (1,) or words:

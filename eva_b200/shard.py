@@ -192,6 +192,8 @@ def _subset(inputs, names):
                 out.set_cipher(name, arr, scale)
             elif kind == "seeded_cipher":      # carried compressed: the instance that stages it expands c1
                 out.set_seeded_cipher(name, arr, inputs.get_seed(name), scale)
+            elif kind == "compact_cipher":     # a response, never an input
+                raise ValueError("input %s is a compact response (compact_outputs): it can only be decrypted" % name)
             elif kind == "stored":             # the entry lives in one server's store; a B200Public has none
                 raise ValueError("input %s is a reference to a stored ciphertext (handle %d): the sharded modes run on B200Public "
                                  "contexts, which have no store; send the ciphertext inline" % (name, arr))
@@ -204,7 +206,7 @@ def _subset(inputs, names):
 
 def run_part(pub, plan, rank, inputs):
     """rank `rank`'s share of the DAG: returns (partial ciphertext [size][ell][N], scale)"""
-    _, partial, scale = pub.execute(plan.parts[rank], _subset(inputs, set(plan.parts[rank].inputs))).get("partial")
+    _, partial, scale = pub.execute_full(plan.parts[rank], _subset(inputs, set(plan.parts[rank].inputs))).get("partial")
     return partial, scale
 
 
@@ -215,7 +217,7 @@ def run_tail(pub, plan, partials, scale, inputs):
     for r, p in enumerate(partials):
         tail_inputs.set_cipher("partial_%d" % r, p, scale)
     try:
-        return pub.execute(plan.tail, tail_inputs)
+        return pub.execute_full(plan.tail, tail_inputs)
     finally:
         pub.set_input_sizes({})
 
@@ -224,11 +226,11 @@ def execute_sharded(pub, prog, inputs, rank=0, world=1, plan=None, device=None):
     """every rank calls this with the same program and inputs (replicated, like the keys): rank r runs
     part r, the partial sums are gathered on rank 0 (the only exchange: NCCL, or gloo on CPU tensors),
     rank 0 runs the tail and returns the outputs (other ranks return None).  Bit-identical to
-    pub.execute(prog, inputs)."""
+    pub.execute(prog, inputs) with compact_outputs off: the sharded modes ignore that option and return full ciphertexts."""
     from . import multi
     plan = plan or split_program(prog, world)
     if world == 1 or plan is None:
-        return pub.execute(prog, inputs) if rank == 0 else None
+        return pub.execute_full(prog, inputs) if rank == 0 else None
     import os
     import time
     t0 = time.perf_counter()

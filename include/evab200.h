@@ -268,6 +268,23 @@ int evab_expand_cipher_uniform(evab_ctx *ctx, int n, const uint8_t *h_seeds, uin
  * several launches on `stream`), so a captured graph replays the copies as they were.  Stream-ordered, does not synchronise;
  * evab_set_batch does not apply.  n >= 0 (0: no launch); the tables must not be null. */
 int evab_gather_ciphers(evab_ctx *ctx, int n, const uint64_t *const *h_src, uint64_t *const *h_dst, const uint64_t *h_words, void *stream);
+/* Compact responses (compact_kernels.cuh; DESIGN §4): n size-2 ciphertexts [2][ell][N] in NTT form at h_src[i] (device, 16-byte
+ * aligned), all with the same ell, switched to the modulus 2^bits and bit-packed into h_dst[i] (device, 8-byte aligned, [2][W] words,
+ * W = ceil(N bits / 64)).  Every coefficient x of c0 and c1 becomes floor((2^(shift+1) x + Q) / (2Q)) mod 2^bits, exactly
+ * (Q = q_0 ... q_{ell-1}).  d_work (16-byte aligned) holds evab_compact_work_bytes(ctx, n, ell) bytes: the coefficient form of the
+ * n ciphertexts.  Launches: ceil(n / 160) gathers into d_work, one inverse transform of the 2 n ell rows and ceil(n / 256)
+ * compactions, whatever the data.  The host tables are read during the call; evab_set_batch does not apply.  Stream-ordered, does
+ * not synchronise.  0 <= n <= 32767 (0: no launch), 1 <= ell <= min(8, k), 1 <= bits <= 62, shift >= bits. */
+size_t evab_compact_work_bytes(const evab_ctx *ctx, int n, int ell);
+int evab_compact_ciphers(evab_ctx *ctx, int n, const uint64_t *const *h_src, uint64_t *const *h_dst, int ell, int shift, int bits, void *d_work,
+                         void *stream);
+/* The client side of a compact value [2][W] at d_words: evab_compact_unpack writes both polynomials' fields as residues modulo the
+ * primes 0 .. nres-1, d_out [2][nres][N] in coefficient form.  evab_compact_finish takes y0 + y1 s in coefficient form over those
+ * nres primes (d_coef [nres][N]; exact when their product exceeds 2 (N+1) 2^bits), reduces it mod 2^bits, centres it to
+ * (-2^(bits-1), 2^(bits-1)] and writes that integer z as residues modulo the primes 0 .. nout-1 (d_out [nout][N], coefficient form)
+ * and, if d_z is not null, as int64 values d_z [N].  1 <= nres, nout <= min(8, k), 1 <= bits <= 62.  Stream-ordered. */
+int evab_compact_unpack(evab_ctx *ctx, const uint64_t *d_words, int bits, int nres, uint64_t *d_out, void *stream);
+int evab_compact_finish(evab_ctx *ctx, const uint64_t *d_coef, int nres, int bits, int nout, uint64_t *d_out, int64_t *d_z, void *stream);
 /* n <= 16 rotations of ONE ciphertext (seal::Evaluator::rotate_vector, seal_executor.h:176-189) in three kernel launches instead of
  * 3 n: d_out [n][2][ell][N], rotation i by galois_elts[i]; same bits as n calls of evab_rotate_modup_prepared.  d_ext, keys, cadds as there. */
 /* evab_rotate_modup_many and evab_lazy_rotsum read P * c0 from the diagonal of d_ext (ext[m][J] has no entry for m = q_J): call this once
