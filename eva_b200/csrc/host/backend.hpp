@@ -280,22 +280,66 @@ private:
   RegionFences fences_;   // of the c1 regions
 };
 
-// Server-resident input ciphertexts (B200Server store_entries): one device allocation of `capacity` entries of 2 (k-1) N words,
-// each holding one tenant's size-2 ciphertext [2][ell][N] at its level.  A request names an entry by handle where it would carry
-// the ciphertext, and staging copies the entry into the arena (evab_gather_ciphers).  Handles increase and are never reused, so a
-// released handle, or one of a tenant whose keys were removed (its entries go with them), names nothing afterwards.  Entries do
-// not depend on key residency.  A fill runs on the store's fill stream and is synchronised before store() returns; it first waits
-// for the gathers that may still read a released entry (the whole store is one region of its RegionFences, read by every gather).
+// Server-resident input ciphertexts (B200Server store_entries, max_stored, store_storage).  A request names an entry by handle
+// where it would carry the ciphertext, and staging copies the entry's device words into the arena (evab_gather_ciphers).  Handles
+// increase and are never reused, so a released handle, or one of a tenant whose keys were removed (its entries go with them),
+// names nothing afterwards.  Entries do not depend on key residency.
+//  - Layout.  "expanded": a device entry holds the size-2 ciphertext [2][ell][N] (2 (k-1) N words).  "seeded" (seeded ciphertexts
+//    only): a device entry holds c0 [ell][N] ((k-1) N words) and the Entry keeps the seed; staging adds the seed to the chunk's
+//    evab_expand_cipher_uniform call, which draws c1 into the arena exactly as for the same ciphertext sent inline.
+//  - Paging (max_stored > store_entries).  Every entry lives in page-locked host memory (a seeded ciphertext as c0 and its seed, in
+//    either layout), and the device entries are the regions of a RegionCache keyed by entry id: store() does no device work, and
+//    every enqueue resolves its batch's entries (assignAll), filling the missing ones on the fill stream (one upload of the host
+//    words; in the expanded layout a seeded entry's c1 is drawn into the region too).  Without paging, entry e is device region e,
+//    written by store() and synchronised before it returns.
+//  - Ordering, per device region (RegionFences): a fill (or a store() into a released region) waits for the gathers that may still
+//    read the region, and a chunk's gather waits for the fills of the regions it reads.
 class CipherStore {
 public:
-  struct Entry { int tenant = -1, ell = 0; double scale = 0; std::uint64_t handle = 0; };   // handle 0: free
-  CipherStore(std::shared_ptr<Device> dev, int capacity)
-      : dev_(std::move(dev)), entries_(capacity), words_(dev_, (std::size_t)capacity * entryWords()), fences_(dev_, 1) {}
-  int capacity() const { return (int)entries_.size(); }
+  struct Entry {
+    int tenant = -1, ell = 0;
+    double scale = 0;
+    std::uint64_t handle = 0;   // 0: free
+    bool seeded = false;        // stored from a seeded ciphertext: `seed` is the seed of its c1
+    KeySeed seed{};
+    HostBuf host;               // paging: the entry's page-locked words, c0 [ell][N] when seeded, else [2][ell][N]
+  };
+  // store_storage: "expanded" or "seeded" (true)
+  static bool seededLayout(const std::string &storage) {
+    if (storage != "expanded" && storage != "seeded")
+      throw std::invalid_argument("store_storage must be \"expanded\" or \"seeded\", not \"" + storage + "\"");
+    return storage == "seeded";
+  }
+  // words of a device entry, and of a paged entry's host copy at ell residues
+  static std::size_t entryWords(int k, u64 N, bool seededLayout) { return (seededLayout ? 1 : 2) * (std::size_t)(k - 1) * N; }
+  static std::size_t hostWords(int ell, u64 N, bool seededCipher) { return (seededCipher ? 1 : 2) * (std::size_t)ell * N; }
+
+  CipherStore(std::shared_ptr<Device> dev, int capacity, int maxStored, bool seeded)
+      : dev_(std::move(dev)), seeded_(seeded), entries_(maxStored), cache_(capacity), words_(dev_, (std::size_t)capacity * entryWords()),
+        fences_(dev_, capacity) {}
+  int capacity() const { return cache_.regions(); }
+  int maxStored() const { return (int)entries_.size(); }
+  bool paged() const { return maxStored() > capacity(); }
+  bool seeded() const { return seeded_; }
   int used() const { return (int)slotOf_.size(); }
-  std::size_t entryWords() const { return 2 * (std::size_t)(dev_->k() - 1) * dev_->N(); }
-  // every value of `v` into a free entry of `tenant`, all or nothing: full size-2 ciphertexts are uploaded, seeded ones have their
-  // c0 uploaded and their c1 drawn into the entry once.  Returns name -> handle
+  std::size_t entryWords() const { return entryWords(dev_->k(), dev_->N(), seeded_); }
+  std::uint64_t fills() const { return paged() ? cache_.fills() : 0; }
+  std::uint64_t evictions() const { return paged() ? cache_.evictions() : 0; }
+  // the handles whose entry holds a device region (paging: in region order)
+  std::vector<std::uint64_t> resident() const {
+    std::vector<std::uint64_t> h;
+    if (paged()) for (int e : cache_.holders()) h.push_back(entries_[e].handle);
+    else for (auto &kv : slotOf_) h.push_back(kv.first);
+    return h;
+  }
+  std::size_t hostBytes() const {
+    std::size_t w = 0;
+    for (const Entry &e : entries_) w += e.host.size();
+    return w * 8;
+  }
+  // every value of `v` into a free entry of `tenant`, all or nothing.  Without paging, full ciphertexts are uploaded, and seeded
+  // ones have their c0 uploaded and (expanded layout) their c1 drawn into the entry once.  With paging the words go to page-locked
+  // host memory only.  Returns name -> handle
   std::map<std::string, std::uint64_t> store(int tenant, const B200Valuation &v) {
     const u64 N = dev_->N();
     const int k = dev_->k();
@@ -304,6 +348,9 @@ public:
       if (auto *c = std::get_if<HostCipher>(&kv.second)) {
         if (c->size != 2 || c->ell < 1 || c->ell > k - 1 || c->data.size() != (std::size_t)2 * c->ell * N)
           throw std::invalid_argument(what + ": only size-2 ciphertexts of the server's parameters can be stored");
+        if (seeded_)
+          throw std::invalid_argument(what + " is a full ciphertext: a store with store_storage=\"seeded\" keeps c0 rows and seeds and takes "
+                                      "seeded ciphertexts only (B200Secret.encrypt)");
       } else if (auto *sc = std::get_if<HostSeededCipher>(&kv.second)) {
         if (sc->ell < 1 || sc->ell > k - 1 || sc->c0.size() != (std::size_t)sc->ell * N)
           throw std::invalid_argument(what + ": seeded ciphertext does not match the server's parameters (level / degree)");
@@ -313,38 +360,50 @@ public:
         throw std::invalid_argument(what + " is " + kind + ": only ciphertexts can be stored");
       }
     }
-    if (capacity() - used() < (int)v.size())
-      throw std::invalid_argument("the ciphertext store has " + std::to_string(capacity() - used()) + " free entries of store_entries=" +
-                                  std::to_string(capacity()) + " and the valuation holds " + std::to_string(v.size()) + ": release entries first");
-    void *stream = fences_.stream();
-    fences_.awaitReaders(0);
-    std::vector<int> slots;
-    for (int i = 0; i < capacity() && slots.size() < v.size(); i++) if (!entries_[i].handle) slots.push_back(i);
-    std::vector<KeySeed> seeds;
-    std::vector<u64 *> c1;
-    std::vector<int> ells;
+    if (maxStored() - used() < (int)v.size())
+      throw std::invalid_argument("the ciphertext store has " + std::to_string(maxStored() - used()) + " free entries of " +
+                                  (paged() ? "max_stored=" : "store_entries=") + std::to_string(maxStored()) + " and the valuation holds " +
+                                  std::to_string(v.size()) + ": release entries first");
+    std::vector<int> ids;
+    for (int e = 0; e < maxStored() && ids.size() < v.size(); e++) if (!entries_[e].handle) ids.push_back(e);
+    std::vector<HostBuf> host(v.size());
+    if (paged()) {   // copied before any entry changes (all or nothing)
+      std::size_t i = 0;
+      for (auto &kv : v) {
+        HostBuf &h = host[i++];
+        if (auto *hc = std::get_if<HostCipher>(&kv.second)) h.assign(hc->data.begin(), hc->data.end());
+        else { auto &sc = std::get<HostSeededCipher>(kv.second); h.assign(sc.c0.begin(), sc.c0.end()); }
+      }
+    } else {         // entry e is device region e
+      void *stream = fences_.stream();
+      std::vector<KeySeed> seeds;
+      std::vector<u64 *> c1;
+      std::vector<int> ells;
+      std::size_t i = 0;
+      for (auto &kv : v) {
+        const int e = ids[i++];
+        u64 *dst = region(e);
+        fences_.awaitReaders(e);
+        if (auto *hc = std::get_if<HostCipher>(&kv.second)) {
+          dev_->upload(dst, hc->data.data(), hc->data.size() * 8, stream);
+        } else {
+          auto &sc = std::get<HostSeededCipher>(kv.second);
+          dev_->upload(dst, sc.c0.data(), sc.c0.size() * 8, stream);
+          if (!seeded_) { seeds.push_back(sc.seed); c1.push_back(dst + sc.c0.size()); ells.push_back(sc.ell); }
+        }
+      }
+      if (!seeds.empty()) expandCiphers(*dev_, (int)seeds.size(), seeds.data(), c1.data(), ells.data(), stream);
+      check(evab_sync(dev_->ctx(), stream));   // the first request that names an entry needs no fill event
+    }
+    std::map<std::string, std::uint64_t> out;
     std::size_t i = 0;
     for (auto &kv : v) {
-      u64 *dst = words_.get() + slots[i++] * entryWords();
-      if (auto *hc = std::get_if<HostCipher>(&kv.second)) {
-        dev_->upload(dst, hc->data.data(), hc->data.size() * 8, stream);
-      } else {
-        auto &sc = std::get<HostSeededCipher>(kv.second);
-        dev_->upload(dst, sc.c0.data(), sc.c0.size() * 8, stream);
-        seeds.push_back(sc.seed); c1.push_back(dst + sc.c0.size()); ells.push_back(sc.ell);
-      }
-    }
-    if (!seeds.empty()) expandCiphers(*dev_, (int)seeds.size(), seeds.data(), c1.data(), ells.data(), stream);
-    check(evab_sync(dev_->ctx(), stream));   // the first request that names an entry needs no fill event
-    std::map<std::string, std::uint64_t> out;
-    i = 0;
-    for (auto &kv : v) {
-      const int slot = slots[i++];
-      Entry &e = entries_[slot];
-      e.tenant = tenant; e.handle = next_++;
+      const int id = ids[i];
+      Entry &e = entries_[id];
+      e.tenant = tenant; e.handle = next_++; e.host = std::move(host[i++]);
       if (auto *hc = std::get_if<HostCipher>(&kv.second)) { e.ell = hc->ell; e.scale = hc->scale; }
-      else { auto &sc = std::get<HostSeededCipher>(kv.second); e.ell = sc.ell; e.scale = sc.scale; }
-      slotOf_[e.handle] = slot;
+      else { auto &sc = std::get<HostSeededCipher>(kv.second); e.ell = sc.ell; e.scale = sc.scale; e.seeded = true; e.seed = sc.seed; }
+      slotOf_[e.handle] = id;
       out[kv.first] = e.handle;
     }
     return out;
@@ -354,36 +413,81 @@ public:
     auto it = slotOf_.find(handle);
     return it == slotOf_.end() ? nullptr : &entries_[it->second];
   }
-  const u64 *words(std::uint64_t handle) const { return words_.get() + (std::size_t)slotOf_.at(handle) * entryWords(); }
+  // the device words of a stored ciphertext: its region, as resolved for the batch being enqueued
+  const u64 *words(std::uint64_t handle) const {
+    const int e = slotOf_.at(handle), r = paged() ? cache_.regionOf(e) : e;
+    if (r < 0) throw std::logic_error("stored ciphertext " + std::to_string(handle) + " staged without a device entry (not resolved)");
+    return region(r);
+  }
   void release(std::uint64_t handle) {
     auto it = slotOf_.find(handle);
     if (it == slotOf_.end()) throw std::invalid_argument("handle " + std::to_string(handle) + " names no stored ciphertext (never issued, or released)");
-    entries_[it->second] = Entry();
+    clear(it->second);
     slotOf_.erase(it);
   }
   void dropTenant(int tenant) {
     for (auto it = slotOf_.begin(); it != slotOf_.end();)
-      if (entries_[it->second].tenant == tenant) { entries_[it->second] = Entry(); it = slotOf_.erase(it); }
+      if (entries_[it->second].tenant == tenant) { clear(it->second); it = slotOf_.erase(it); }
       else ++it;
   }
-  // `stream` has enqueued gathers from the store: a later fill waits for them
-  void afterGather(void *stream) {
-    const int store = 0;
-    fences_.afterRun(stream, &store, 1);
+  // The device region of every stored reference of the instances inputs[0 .. n), instance b's at [from[b], from[b + 1]) in the
+  // order stageInputs meets them (references checked by checkStored).  With paging, the missing entries' fills are enqueued on the
+  // fill stream
+  std::vector<int> resolve(const B200Valuation *const *inputs, int n, std::vector<int> &from) {
+    std::vector<int> ids;
+    from.assign(1, 0);
+    for (int b = 0; b < n; b++) {
+      for (auto &in : *inputs[b])
+        if (auto *r = std::get_if<StoredCipher>(&in.second)) ids.push_back(slotOf_.at(r->handle));
+      from.push_back((int)ids.size());
+    }
+    if (!paged() || ids.empty()) return ids;
+    std::vector<RegionCache::Fill> fills;
+    std::vector<int> regions = cache_.assignAll(ids, fills);
+    void *stream = fences_.stream();
+    std::vector<KeySeed> seeds;
+    std::vector<u64 *> c1;
+    std::vector<int> ells;
+    for (auto &f : fills) {
+      const Entry &e = entries_[f.tenant];
+      u64 *dst = region(f.region);
+      fences_.awaitReaders(f.region);
+      dev_->upload(dst, e.host.data(), e.host.size() * 8, stream);
+      if (e.seeded && !seeded_) { seeds.push_back(e.seed); c1.push_back(dst + e.host.size()); ells.push_back(e.ell); }
+    }
+    if (!seeds.empty()) expandCiphers(*dev_, (int)seeds.size(), seeds.data(), c1.data(), ells.data(), stream);
+    for (auto &f : fills) fences_.filled(f.region);
+    return regions;
   }
+  // a chunk on `stream` that gathers from `regions` waits for their fills; once enqueued, it is recorded as their reader
+  void beforeRun(void *stream, const int *regions, int n) { fences_.beforeRun(stream, regions, n); }
+  void afterRun(void *stream, const int *regions, int n) { fences_.afterRun(stream, regions, n); }
 
 private:
+  u64 *region(int r) const { return words_.get() + (std::size_t)r * entryWords(); }
+  // entry e is free again: with paging its device copy is dropped, and its host words freed once no fill reads them
+  void clear(int e) {
+    if (paged()) {
+      cache_.drop(e);
+      check(evab_sync(dev_->ctx(), fences_.stream()));
+    }
+    entries_[e] = Entry();
+  }
   std::shared_ptr<Device> dev_;
-  std::vector<Entry> entries_;
-  DBuf words_;                                      // [capacity][2 (k-1) N]
-  RegionFences fences_;                             // region 0: words_ (destroyed first: its fills write words_)
+  bool seeded_;                                     // store_storage="seeded"
+  std::vector<Entry> entries_;                      // [max_stored]
+  RegionCache cache_;                               // paging: the entry held by each device region
+  DBuf words_;                                      // [store_entries][entryWords()]
+  RegionFences fences_;                             // of the device regions (destroyed first: its fills read entries_ and write words_)
   std::map<std::uint64_t, int> slotOf_;             // live handle -> entry
   std::uint64_t next_ = 1;
 };
 
-// where every instance of a batch reads its keys: its key-bank slot (empty: no key bank) and its c1 table entry (empty: no c1 cache)
+// where every instance of a batch reads its keys: its key-bank slot (empty: no key bank) and its c1 table entry (empty: no c1
+// cache); and the store regions its stored inputs are gathered from, instance b's stored[storedFrom[b] .. storedFrom[b + 1])
+// (storedFrom empty: no store)
 struct Residency {
-  std::vector<int> slots, c1;
+  std::vector<int> slots, c1, stored, storedFrom;
   const int *c1At(int b0) const { return c1.empty() ? nullptr : c1.data() + b0; }
 };
 
@@ -397,21 +501,26 @@ struct Shared {
   std::unique_ptr<CipherStore> store;   // B200Server with store_entries > 0: the tenants' stored input ciphertexts
   std::mutex execMutex;   // serialises execute / executeMany callers of one context (see executeMany), and key-bank changes
   void requireTenant(int t) const { if (pager) pager->requireRegistered(t); else bank->requireOccupied(t); }
-  // the residency of every instance (with paging and a c1 cache: resolved, and the missing tenants' fills enqueued, slots first)
-  Residency resolve(const std::vector<int> &tenants) {
+  // the residency of every instance, and of the stored inputs of inputs[0 .. n) when given (with paging and a c1 cache: resolved,
+  // and the missing fills enqueued: slots, c1 rows, store entries)
+  Residency resolve(const std::vector<int> &tenants, const B200Valuation *const *inputs = nullptr, int n = 0) {
     Residency r;
     r.slots = pager ? pager->resolve(tenants) : tenants;
     if (c1) r.c1 = c1->resolve(tenants, r.slots);
+    if (store && inputs) r.stored = store->resolve(inputs, n, r.storedFrom);
     return r;
   }
-  // a run on `stream` of instances b0 .. b0 + nb waits for the fills of what they read; once enqueued, it is recorded as its reader
+  // the staging and the run on `stream` of instances b0 .. b0 + nb wait for the fills of what they read; once enqueued, they are
+  // recorded as its reader
   void beforeRun(void *stream, const Residency &r, int b0, int nb) {
     if (pager) pager->beforeRun(stream, r.slots.data() + b0, nb);
     if (c1) c1->beforeRun(stream, r.c1.data() + b0, nb);
+    if (!r.storedFrom.empty()) store->beforeRun(stream, r.stored.data() + r.storedFrom[b0], r.storedFrom[b0 + nb] - r.storedFrom[b0]);
   }
   void afterRun(void *stream, const Residency &r, int b0, int nb) {
     if (pager) pager->afterRun(stream, r.slots.data() + b0, nb);
     if (c1) c1->afterRun(stream, r.c1.data() + b0, nb);
+    if (!r.storedFrom.empty()) store->afterRun(stream, r.stored.data() + r.storedFrom[b0], r.storedFrom[b0 + nb] - r.storedFrom[b0]);
   }
 };
 
@@ -521,7 +630,8 @@ public:
   // Client-supplied valuations are untrusted (they may come from a file): every buffer is checked against the shape the plan
   // expects before its copy.  A seeded ciphertext's c0 is uploaded like any other input; the c1 rows of all of the chunk's seeded
   // ciphertexts are then expanded on the device by one evab_expand_cipher_uniform call.  The chunk's stored inputs (references
-  // checked by checkStored before the batch was enqueued) are copied from the store by one evab_gather_ciphers call.
+  // checked by checkStored and resolved before the batch was enqueued) are copied from the store by one evab_gather_ciphers call:
+  // whole entries, or with store_storage="seeded" their c0 rows, whose seeds join the expansion call.
   void stageInputs(Executor &ex, Program &program, const B200Valuation *const *inputs, int nb, void *stream) {
     const u64 N = s_->dev->N();
     std::vector<KeySeed> seeds;
@@ -545,8 +655,17 @@ public:
           s_->dev->upload(dst, sc->c0.data(), sc->c0.size() * 8, stream);
           seeds.push_back(sc->seed); c1.push_back(dst + sc->c0.size()); ells.push_back(sc->ell);
         } else if (auto *r = std::get_if<StoredCipher>(&in.second)) {
-          if (!s_->store || !s_->store->find(r->handle)) throw std::logic_error("input " + in.first + ": stored reference staged without checkStored");
-          gatherSrc.push_back(s_->store->words(r->handle)); gatherDst.push_back(ex.valuePtr(term, b)); gatherWords.push_back((u64)2 * vi.ell * N);
+          const CipherStore::Entry *e = s_->store ? s_->store->find(r->handle) : nullptr;
+          if (!e) throw std::logic_error("input " + in.first + ": stored reference staged without checkStored");
+          u64 *dst = ex.valuePtr(term, b);
+          const std::size_t c0 = (std::size_t)vi.ell * N;
+          gatherSrc.push_back(s_->store->words(r->handle)); gatherDst.push_back(dst);
+          if (s_->store->seeded()) {
+            gatherWords.push_back(c0);
+            seeds.push_back(e->seed); c1.push_back(dst + c0); ells.push_back(vi.ell);
+          } else {
+            gatherWords.push_back(2 * c0);
+          }
         } else if (std::holds_alternative<HostCompactCipher>(in.second)) {
           throw compactRefused("input " + in.first);
         } else if (auto *p = std::get_if<HostPlain>(&in.second)) {
@@ -564,17 +683,18 @@ public:
     // One launch for the chunk, on the chunk's stream, before its run.  Stream order gives the rest: the expansion starts after the
     // replica's previous run has stopped reading the arena, a collect() redo (the zero-digit case) stages again and so expands the
     // same words again, and a packed arena never lends an input's storage to another value (inputs are pinned).  The same holds
-    // for the gather of stored inputs, whose entries cannot be released while a batch that names them is uncollected.
+    // for the gather of stored inputs, whose entries cannot be released while a batch that names them is uncollected; the caller
+    // orders it against the fills of the entries' device regions (Shared::beforeRun / afterRun).
     if (!seeds.empty()) expandCiphers(*s_->dev, (int)seeds.size(), seeds.data(), c1.data(), ells.data(), stream);
-    if (!gatherSrc.empty()) {
+    if (!gatherSrc.empty())
       check(evab_gather_ciphers(s_->dev->ctx(), (int)gatherSrc.size(), gatherSrc.data(), gatherDst.data(), gatherWords.data(), stream));
-      s_->store->afterGather(stream);
-    }
   }
   // Stored inputs come from outside the program as much as inline ones.  Before anything of a batch is enqueued, every reference
   // is checked: the handle names an entry, the entry belongs to the tenant of the instance that names it (tenants[b]; null without
-  // a key bank), and its level and size are the input's in the plan, as stageInputs checks an inline ciphertext
+  // a key bank), and its level and size are the input's in the plan, as stageInputs checks an inline ciphertext.  With paging, the
+  // batch names at most store_entries distinct entries (all of them are on the device while it is staged)
   void checkStored(const Executor &ex, Program &program, const B200Valuation *const *inputs, const int *tenants, int nb) const {
+    std::set<std::uint64_t> distinct;
     for (int b = 0; b < nb; b++)
       for (auto &in : *inputs[b]) {
         auto *r = std::get_if<StoredCipher>(&in.second);
@@ -589,7 +709,12 @@ public:
         if (vi.kind != Kind::Cipher || vi.size != 2 || vi.ell != e->ell)
           throw std::invalid_argument(what + who + ": the stored ciphertext (size 2, ell " + std::to_string(e->ell) + ") does not match the program signature (" +
                                       (vi.kind == Kind::Cipher ? "size " + std::to_string(vi.size) + ", ell " + std::to_string(vi.ell) : std::string("not a ciphertext")) + ")");
+        distinct.insert(r->handle);
       }
+    if (s_->store && (int)distinct.size() > s_->store->capacity())
+      throw std::invalid_argument("a batch names " + std::to_string(distinct.size()) + " distinct stored ciphertexts but the store has store_entries=" +
+                                  std::to_string(s_->store->capacity()) + " device entries (max_stored=" + std::to_string(s_->store->maxStored()) +
+                                  "): split the batch");
   }
   // with execMutex held: does a submitted, not yet collected batch name this stored ciphertext?
   bool storedInFlightLocked(std::uint64_t handle) const {
@@ -705,8 +830,9 @@ public:
       checkStored(first, program, inputs.data(), p.tenants.empty() ? nullptr : p.tenants.data(), B);
     }
     std::vector<char> busy(R, 0);
-    // residency of every instance, resolved at every enqueue (so that collect's redo refills a tenant evicted meanwhile)
-    const Residency res = s_->resolve(p.tenants);
+    // residency of every instance and stored input, resolved at every enqueue (so that collect's redo refills a tenant or a stored
+    // ciphertext evicted meanwhile)
+    const Residency res = s_->resolve(p.tenants, inputs.data(), B);
     for (int b0 = 0, g = 0; b0 < B; b0 += F, g++) {
       const int nb = std::min(F, B - b0);
       const int r = g % R;
@@ -720,9 +846,9 @@ public:
       if (std::find(streams.begin(), streams.end(), st) == streams.end()) streams.push_back(st);
       if (std::find(p.plans.begin(), p.plans.end(), holder) == p.plans.end()) p.plans.push_back(holder);
       auto t1 = now();
+      s_->beforeRun(st, res, b0, nb);
       stageInputs(ex, program, inputs.data() + b0, nb, st);
       auto t2 = now();
-      s_->beforeRun(st, res, b0, nb);
       ex.run(st);
       s_->afterRun(st, res, b0, nb);
       if (p.compact) compactOutputsOf(*holder, program, p.compact, outs.data() + b0, nb, st);
@@ -811,11 +937,20 @@ public:
   // inside the key-switch inner products (KeyBank).  keyStorage: "expanded" -- every key in full; "seeded" (inline constants only) --
   // c0 rows and seeds, the key switches draw the c1 rows (KeyBank).  c1Cache (seeded keys, 0 .. capacity): regions holding the
   // expanded c1 rows of the tenants used most (C1Store); 0 is the plain seeded bank
-  // storeEntries: entries of the ciphertext store (CipherStore), 0 for none
+  // storeEntries: device entries of the ciphertext store (CipherStore), 0 for none.  maxStored < 0 or == storeEntries: every stored
+  // ciphertext holds a device entry; maxStored > storeEntries: up to maxStored in page-locked host memory, paged into the device
+  // entries.  storeStorage: "expanded" -- device entries hold whole ciphertexts; "seeded" -- c0 rows and seeds of seeded ciphertexts
   B200Server(const CKKSParameters &params, int capacity, int device, int maxTenants = -1, const std::string &rotationKeys = "program",
-             const std::string &hoistConstants = "stored", const std::string &keyStorage = "expanded", int c1Cache = 0, int storeEntries = 0)
-      : rotationKeys_(rotationKeys), hoistConstants_(hoistConstants), keyStorage_(keyStorage) {
+             const std::string &hoistConstants = "stored", const std::string &keyStorage = "expanded", int c1Cache = 0, int storeEntries = 0,
+             int maxStored = -1, const std::string &storeStorage = "expanded")
+      : rotationKeys_(rotationKeys), hoistConstants_(hoistConstants), keyStorage_(keyStorage), storeStorage_(storeStorage) {
     if (storeEntries < 0) throw std::invalid_argument("store_entries (" + std::to_string(storeEntries) + ") must be >= 0");
+    const bool seededStore = CipherStore::seededLayout(storeStorage);
+    if (maxStored >= 0 && maxStored < storeEntries)
+      throw std::invalid_argument("max_stored (" + std::to_string(maxStored) + ") is below the number of device entries (store_entries " +
+                                  std::to_string(storeEntries) + ")");
+    if (maxStored > 0 && storeEntries == 0)
+      throw std::invalid_argument("max_stored (" + std::to_string(maxStored) + ") pages stored ciphertexts into device entries: it needs store_entries > 0");
     if (hoistConstants != "stored" && hoistConstants != "inline")
       throw std::invalid_argument("hoist_constants must be \"stored\" or \"inline\", not \"" + hoistConstants + "\"");
     if (keyStorage != "expanded" && !(keyStorage == "seeded" && hoistConstants == "inline"))
@@ -842,10 +977,11 @@ public:
     s->bank = std::make_unique<KeyBank>(s->dev, elts, capacity, hoistConstants == "inline", keyStorage == "seeded", c1Cache);
     if (maxTenants > capacity) s->pager = std::make_unique<KeyPager>(s->dev, *s->bank, maxTenants);
     if (c1Cache > 0) s->c1 = std::make_unique<C1Store>(s->dev, *s->bank, s->pager.get());
-    if (storeEntries > 0) s->store = std::make_unique<CipherStore>(s->dev, storeEntries);
+    if (storeEntries > 0) s->store = std::make_unique<CipherStore>(s->dev, storeEntries, std::max(maxStored, storeEntries), seededStore);
     pub_ = std::make_unique<B200Public>(s);
   }
-  // the ciphertexts of `enc` (full or seeded) into the store as `tenant`'s entries, all or nothing: name -> handle
+  // the ciphertexts of `enc` (full or seeded; seeded only with store_storage="seeded") into the store as `tenant`'s entries, all or
+  // nothing: name -> handle.  With paging into host memory only (no device work)
   std::map<std::string, std::uint64_t> store(int tenant, const B200Valuation &enc) {
     std::lock_guard<std::mutex> guard(shared()->execMutex);
     requireStore();
@@ -901,8 +1037,11 @@ public:
     for (auto &r : rq) in.push_back(r.second);
     pub_->checkStored(ex, prog, in.data(), tenants.data(), (int)in.size());
     staged_[&ex] = tenants;
-    setKeyTable(ex, shared()->resolve(tenants), stream);
+    const Residency res = shared()->resolve(tenants, in.data(), (int)in.size());
+    setKeyTable(ex, res, stream);
+    shared()->beforeRun(stream, res, 0, (int)in.size());
     pub_->stageInputs(ex, prog, in.data(), (int)in.size(), stream);
+    shared()->afterRun(stream, res, 0, (int)in.size());
   }
   // tenants: replaces the staged tenants of the replica (same count)
   void runResident(Program &prog, void *stream, int batch, int replica, const std::vector<int> &tenants = {}) {
@@ -939,6 +1078,7 @@ public:
   const std::string &rotationKeys() const { return rotationKeys_; }
   const std::string &hoistConstants() const { return hoistConstants_; }
   const std::string &keyStorage() const { return keyStorage_; }
+  const std::string &storeStorage() const { return storeStorage_; }
   std::shared_ptr<Shared> shared() const { return pub_->shared(); }
 
 private:
@@ -952,7 +1092,7 @@ private:
     shared()->dev->sync(stream);
     ex.setKeyTable(res.slots.data(), res.c1At(0), n);
   }
-  std::string rotationKeys_, hoistConstants_, keyStorage_;
+  std::string rotationKeys_, hoistConstants_, keyStorage_, storeStorage_;
   std::unique_ptr<B200Public> pub_;
   std::map<const Executor *, std::vector<int>> staged_;   // device-resident hooks: the tenants staged on a plan replica
 };

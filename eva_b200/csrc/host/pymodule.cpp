@@ -210,6 +210,11 @@ PYBIND11_MODULE(_eva_b200, m) {
         py::arg("slots"), py::arg("batches"));
   m.def("_c1_cache", [=](int regions, const std::vector<py::object> &ops) { return replayRegionCache(regions, ops, false); },
         py::arg("regions"), py::arg("batches"));
+  // test hook: the ciphertext store's layout (CipherStore) without a device: (store_entry_bytes for k primes at degree N, the host
+  // bytes of a paged entry at ell residues, seeded: stored from a seeded ciphertext)
+  m.def("_store_bytes", [](int k, u64 N, const std::string &storeStorage, int ell, bool seeded) {
+    return py::make_tuple(CipherStore::entryWords(k, N, CipherStore::seededLayout(storeStorage)) * 8, CipherStore::hostWords(ell, N, seeded) * 8);
+  }, py::arg("k"), py::arg("N"), py::arg("store_storage"), py::arg("ell"), py::arg("seeded"));
   // test hook: the planner alone (host/planner.hpp), without a device.  options: set_options' keywords; arena_limit 0 is no limit
   // here.  The scratch sizes are stand-ins derived from N and ell (the layout's invariants hold for any sizes)
   py::class_<ExecOptions> planOptions(m, "_PlanOptions");
@@ -579,11 +584,13 @@ PYBIND11_MODULE(_eva_b200, m) {
                              "Executes compiled programs for many clients: each client's evaluation keys are a tenant of a key bank of fixed "
                              "capacity, the plans are shared by all tenants, and every instance of a batch runs with its own tenant's keys");
   srv.def(py::init([](const CKKSParameters &params, int capacity, int device, std::optional<int> maxTenants, const std::string &rotationKeys,
-                       const std::string &hoistConstants, const std::string &keyStorage, int c1Cache, int storeEntries) {
+                       const std::string &hoistConstants, const std::string &keyStorage, int c1Cache, int storeEntries, std::optional<int> maxStored,
+                       const std::string &storeStorage) {
         return std::make_unique<B200Server>(params, capacity, device, maxTenants ? *maxTenants : -1, rotationKeys, hoistConstants, keyStorage, c1Cache,
-                                            storeEntries);
+                                            storeEntries, maxStored ? *maxStored : -1, storeStorage);
       }), py::arg("params"), py::arg("capacity") = 64, py::arg("device") = 0, py::arg("max_tenants") = py::none(), py::arg("rotation_keys") = "program",
       py::arg("hoist_constants") = "stored", py::arg("key_storage") = "expanded", py::arg("c1_cache") = 0, py::arg("store_entries") = 0,
+      py::arg("max_stored") = py::none(), py::arg("store_storage") = "expanded",
       "capacity: device slots (key-bank regions).  max_tenants None or == capacity: a tenant id is its slot, filled when its keys are "
       "added.  max_tenants > capacity: up to max_tenants tenants' keys in page-locked host memory, paged into the slots (least "
       "recently used first) as batches need them.  rotation_keys: the Galois keys every tenant supplies -- \"program\", one per "
@@ -596,7 +603,12 @@ PYBIND11_MODULE(_eva_b200, m) {
       "capacity): device regions, each holding the expanded c1 rows of one tenant; the instances of a batch whose tenant holds one read "
       "them instead of drawing (same outputs).  The tenants with the most instances in a batch are admitted first, the least recently "
       "used region is evicted; tenants without a region draw.  store_entries: device entries of the ciphertext store, each holding "
-      "one stored size-2 input ciphertext (store / release; 0: no store)")
+      "one stored size-2 input ciphertext (store / release; 0: no store).  max_stored None or == store_entries: every stored "
+      "ciphertext holds a device entry.  max_stored > store_entries: up to max_stored stored ciphertexts in page-locked host memory, "
+      "paged into the device entries (least recently used first) as batches name them; a batch names at most store_entries "
+      "distinct ones.  store_storage: \"expanded\", device entries hold whole ciphertexts (a seeded one is expanded when it is "
+      "written to the device); \"seeded\", seeded ciphertexts only (B200Secret.encrypt), entries hold c0 rows and the seed and "
+      "staging draws the uniform half (same outputs, half the entry)")
       .def("add_raw_keys", [](B200Server &s, const u64arr &relin, const std::map<u64, u64arr> &galois) {
         const std::size_t kk = s.shared()->dev->k(), N = s.shared()->dev->N();
         requireShape(relin, {kk - 1, 2, kk, N}, "relinearization key");
@@ -670,9 +682,11 @@ PYBIND11_MODULE(_eva_b200, m) {
          "expanded from seeds (generate_keys, or a loaded compressed context), in full (add_raw_keys) otherwise")
       .def("remove_keys", &B200Server::removeKeys, py::arg("tenant"), "also releases the tenant's stored ciphertexts")
       .def("store", &B200Server::store, py::arg("tenant"), py::arg("enc"), py::call_guard<py::gil_scoped_release>(),
-           "keep the ciphertexts of `enc` (B200Public.encrypt or B200Secret.encrypt; every value a ciphertext) on the device as the "
-           "tenant's entries, all or nothing; a seeded one is expanded once here.  Returns {name: handle}: a request names an entry "
-           "with B200Valuation.set_stored(name, handle), and its outputs are those of the same ciphertext sent inline")
+           "keep the ciphertexts of `enc` (B200Public.encrypt or B200Secret.encrypt; every value a ciphertext; with "
+           "store_storage=\"seeded\" B200Secret.encrypt only) as the tenant's entries, all or nothing: on the device (with "
+           "store_storage=\"expanded\" a seeded one is expanded once here), or with max_stored > store_entries in page-locked host "
+           "memory only, a seeded one as c0 rows and seed.  Returns {name: handle}: a request names an entry with "
+           "B200Valuation.set_stored(name, handle), and its outputs are those of the same ciphertext sent inline")
       .def("release", &B200Server::release, py::arg("handle"), "free a stored ciphertext's entry; its handle names nothing afterwards")
       .def("execute", [](B200Server &s, Program &prog, int tenant, const B200Valuation &in) {
         return std::move(s.executeBatch(prog, {{tenant, &in}})[0]);
@@ -727,9 +741,15 @@ PYBIND11_MODULE(_eva_b200, m) {
         d["c1_fills"] = c1 ? c1->cache().fills() : 0;
         d["c1_evictions"] = c1 ? c1->cache().evictions() : 0;
         const CipherStore *st = s.cipherStore();
-        const std::size_t entryBytes = 2 * (std::size_t)(s.shared()->dev->k() - 1) * s.shared()->dev->N() * 8;
+        const std::size_t entryBytes = CipherStore::entryWords(s.shared()->dev->k(), s.shared()->dev->N(), CipherStore::seededLayout(s.storeStorage())) * 8;
         d["store_entries"] = st ? st->capacity() : 0;
+        d["max_stored"] = st ? st->maxStored() : 0;
+        d["store_storage"] = s.storeStorage();
         d["stored"] = st ? st->used() : 0;
+        d["store_resident"] = st ? st->resident() : std::vector<std::uint64_t>();
+        d["store_fills"] = st ? st->fills() : 0;
+        d["store_evictions"] = st ? st->evictions() : 0;
+        d["store_host_bytes"] = st ? st->hostBytes() : 0;
         d["store_entry_bytes"] = entryBytes;
         d["store_bytes"] = st ? entryBytes * (std::size_t)st->capacity() : 0;
         return d;
@@ -741,7 +761,12 @@ PYBIND11_MODULE(_eva_b200, m) {
          "compressed_tenants: tenants added in compressed form; fills: slots filled (keys uploaded and "
          "constants computed); evictions: resident tenants displaced by a fill; c1_cache: c1 regions (c1_cache_bytes of device memory); "
          "c1_cached: the tenants holding one; c1_fills: regions expanded; c1_evictions: cached tenants displaced by a fill; "
-         "store_entries: entries of the ciphertext store (store_bytes of device memory, store_entry_bytes each); stored: entries in use")
+         "store_entries: device entries of the ciphertext store (store_bytes of device memory, store_entry_bytes each: 2 (k-1) N words "
+         "with store_storage \"expanded\", (k-1) N with \"seeded\"); max_stored: stored ciphertexts it can hold (more than "
+         "store_entries: paging); stored: entries in use; store_resident: the handles holding a device entry; store_fills: device "
+         "entries written from host memory (paging); store_evictions: resident entries displaced by a fill; store_host_bytes: "
+         "page-locked host memory of the paged entries (2 ell N words each, ell N for a seeded ciphertext, whose seed is kept "
+         "beside them)")
       .def("primes", [](B200Server &s) { return s.shared()->dev->primes(); })
       // ---- benchmark hooks (as B200Public's): device-resident execution of requests staged on a plan replica
       .def("stage_inputs", [](B200Server &s, Program &prog, const Requests &rq, std::uintptr_t stream, int replica) {
